@@ -4,7 +4,7 @@
     python bench.py [--gpus N] [--steps K] [--warmup W] [--batch B] [--impl ours|reference] [--model 8b|1b|tiny]
 
 A "step" is one decode step of the whole batch (B generated tokens) of BASELINE.json configs[2]
-("Llama-3-8B generate_batch INT8, seq 2048, bsz 1 and 32, on 1xB200"): prompt P=1024 then K generated
+("Llama-3-8B generate_batch INT8, seq 2048, bsz 1 and 32, on 1xH100"): prompt P=1024 then K generated
 tokens per sequence.  One JSON line on stdout (rank 0):
   value    = B*K*N / device time of K decode steps, inputs already resident in HBM (CUDA events, max over ranks)
   e2e      = the same tokens/s through ctranslate2_b200.Generator.generate_batch with HOST prompt ids and HOST
@@ -15,7 +15,7 @@ tokens per sequence.  One JSON line on stdout (rank 0):
              reference's own CUDA build (oracle/_ref_cuda: cuBLAS INT8 GEMM / its AWQ kernels) on the same GPU
   translate = BASELINE.json configs[1] (OPUS-MT-shaped Transformer-base INT8, 64 sentences, beam 4): device-timed decoding
              steps, end-to-end target tokens/s through Translator.translate_batch, beside the reference's CUDA Translator
-  roofline = the weight-streaming tcgen05 GEMM timed alone with CUDA events over buffers larger than L2
+  roofline = the weight-streaming wgmma GEMM timed alone with CUDA events over buffers larger than L2
   cpu_baseline = the unmodified reference (oracle/_ref, Ruy INT8) on the host cores, bounded sample
 N>1: independent data-parallel replicas (one process per GPU, no data-path collective): scaling "weak"; the same line
 also carries `tp`: ONE tensor-parallel generator over the N GPUs (heads / FFN columns sharded, collectives fused into
@@ -69,7 +69,7 @@ def prompts_for(name, batch, plen, seed=42):
 
 
 class ClockSampler:
-    """nvidia-smi clocks/throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks/throttle reasons during the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -123,7 +123,7 @@ def measured_peaks():
     if os.path.exists(p):
         j = json.load(open(p))
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 
 def step_bytes(name, batch, ctx, weights="int8"):
@@ -143,8 +143,8 @@ def step_bytes(name, batch, ctx, weights="int8"):
 
 
 def gemm_roofline(name, batch, device):
-    """Times the dominant kernel (fused gate/up INT8 GEMM on tcgen05, weight streaming) alone with CUDA
-    events, cycling through more weight copies than fit in L2 (126 MB) so every launch streams from HBM."""
+    """Times the dominant kernel (fused gate/up INT8 GEMM on wgmma, weight streaming) alone with CUDA
+    events, cycling through more weight copies than fit in L2 (50 MB) so every launch streams from HBM."""
     import torch
     from ctranslate2_b200 import ops
     m = MODELS[name]
@@ -170,10 +170,7 @@ def gemm_roofline(name, batch, device):
     alg = 2 * f * d + 2 * f * 4 + batch * d + batch * 4 + batch * f * 2    # weights + scales + x + h(out)
     peak, how = measured_peaks()
     ach = alg / (ms * 1e-3) / 1e9
-    # dram__bytes_read.sum + dram__bytes_write.sum of this kernel in the committed ncu --set full capture
-    # (profiles/r02_ncu_final_gemm_decode.md, the final kernel: 117,725,952 B read + 4,043,008 B written at m = 32; round 1's
-    # capture of the first lean kernel read 121,676,544 B in total); null for shapes that were not captured
-    traffic = 121768960 if (name == "8b" and batch == 32) else None
+    traffic = None                # DRAM bytes of the kernel from a profiler capture: none taken on the H100
     return {"bound": "hbm", "kernel": "gemm_decode_kernel<s8, NB=2 gate/up + SwiGLU> (ffn gate/up %dx%d, m=%d)" % (2 * f, d, batch),
             "achieved": round(ach, 1), "peak": peak, "unit": "GB/s", "frac": round(ach / peak, 4),
             "traffic": traffic, "bytes_per_launch": alg, "us_per_launch": round(ms * 1e3, 2), "peak_source": how}
@@ -212,7 +209,7 @@ def awq_roofline(name, batch, device):
     return {"bound": "hbm", "kernel": "awq_decode_kernel<NB=2 gate/up + SwiGLU> (ffn gate/up %dx%d int4 g128, m=%d)" % (2 * f, d, batch),
             "achieved": round(ach, 1), "peak": peak, "unit": "GB/s", "frac": round(ach / peak, 4), "traffic": None,
             "bytes_per_launch": alg, "us_per_launch": round(ms * 1e3, 2), "peak_source": how,
-            "note": "transform (int4 -> fp16) bound, not HBM bound: see profiles/r01_ncu_awq_and_prefill.md"}
+            "note": "the int4 -> fp16 conversion shares the SM with the stream"}
 
 
 def _ref_thread_cache():
@@ -420,13 +417,15 @@ def measure_variant(ct2, torch, name, weights, batch, plen, steps, warmup, devic
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    # default = the named workload: 1024 generated tokens after the 1024-token prompt ("seq 2048"); a few seconds on a B200
+    # default = the named workload: 1024 generated tokens after the 1024-token prompt ("seq 2048"); a few seconds on an H100
     ap.add_argument("--steps", type=int, default=1024)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--batch", type=int, default=32)
     ap.add_argument("--impl", default="ours")
     ap.add_argument("--model", default="8b", choices=list(MODELS))
     ap.add_argument("--prompt-len", type=int, default=PROMPT_LEN)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed decode step computed (logits [batch, vocab], float32) to DIR/logits.npy")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-graph", action="store_true")
     ap.add_argument("--no-variants", action="store_true", help="skip the INT8/AWQ x bsz 1/32 sub-records and ref_cuda")
@@ -451,9 +450,11 @@ def main():
               "global_batch": B * (1 if args.tp else max(1, world)), "prompt_len": P,
               "parallelism": ("tp%d (heads / FFN columns sharded, collectives fused into kernels over NVLink peer memory)" % world)
               if args.tp and world > 1 else "dp%d (replicas, no collective)" % world,
-              "l2": "every step streams %.1f GB of weights (> 126 MB L2) — no flush needed" % (step_bytes(args.model, 0, 0, args.weights) / 1e9)}
+              "l2": "every step streams %.1f GB of weights (> 50 MB L2) — no flush needed" % (step_bytes(args.model, 0, 0, args.weights) / 1e9)}
 
     if args.impl == "reference":
+        if args.dump_outputs:
+            ap.error("--dump-outputs records the GPU path; it has no meaning with --impl reference")
         if rank != 0:
             return
         r = reference_cpu(args.model, B, K, W)
@@ -511,6 +512,10 @@ def main():
     with ClockSampler(local_rank) as clocks:
         pre_ms, dec_ms, launches = gen.bench_decode(B, P, K, W)
         sync_all()
+    if args.dump_outputs and rank == 0:
+        # the prompt ids are a fixed function of their position, so two builds see identical inputs
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "logits.npy"), gen.bench_last_logits(B, MODELS[args.model]["vocab_size"]))
     dec_ms, pre_ms = max_over_ranks(dec_ms, pre_ms)
     value = B * K * units / (dec_ms * 1e-3)
 
@@ -546,8 +551,8 @@ def main():
         line = {"metric": "generate_batch tokens/sec", "value": round(value, 2), "unit": "tokens/s", "n_gpus": world,
                 "steps": K, "warmup": W, "ms_per_step": round(dec_ms / K, 4), "higher_is_better": True,
                 "scaling": "strong" if tp else "weak", "vs_baseline": None,
-                "dtype": ("s4 weights -> f16 (tcgen05 kind::f16, f32 accumulate)" if awq else
-                          "s8 (int8 x int8 -> s32 on tcgen05; f16 activations, f32 epilogue/softmax)"),
+                "dtype": ("s4 weights -> f16 (wgmma f16, f32 accumulate)" if awq else
+                          "s8 (int8 x int8 -> s32 on wgmma; f16 activations, f32 epilogue/softmax)"),
                 "data": "synthetic", "config": config, "clocks": clocks.summary(), "e2e": e2e,
                 "gpu_launches": int(launches)}
         if e2e_full is not None:

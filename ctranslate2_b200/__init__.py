@@ -1,7 +1,7 @@
-"""ctranslate2_b200 — the B200-native (sm_100a) quantized-transformer decode path behind CTranslate2's
+"""ctranslate2_b200 — the H100-native (sm_90a) quantized-transformer decode path behind CTranslate2's
 Generator / ops surface.  Host-side mirror of the reference interface over the C-ABI in include/ct2b200.h.
 There is no CPU or PyTorch fallback: importing works anywhere, every compute call needs libct2b200.so and a
-B200."""
+H100."""
 from . import ops  # noqa: F401
 from ._lib import Ct2B200Error, kernel_launch_count, lib  # noqa: F401
 from .generator import GenerationResult, Generator, model_summary  # noqa: F401

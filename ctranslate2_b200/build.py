@@ -1,4 +1,4 @@
-"""In-tree build of libct2b200.so for sm_100a (cross-compiles without a GPU).
+"""In-tree build of libct2b200.so for sm_90a (cross-compiles without a GPU).
 
     python -m ctranslate2_b200.build [--force]
 
@@ -20,23 +20,20 @@ SOURCES = [
     "kernels/decode_loop.cu", "kernels/seq2seq.cu", "host/engine.cc", "host/beam.cc", "host/translator.cc", "c_api.cc",
 ]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC",
          "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr", "-x", "cu"]
 
 
 # No read-only-path loads (ld.global.nc): nvcc emits them for `const T* __restrict__` kernel parameters, on the promise that the
 # data is not written while the kernel is alive.  Under programmatic dependent launch a kernel is alive BEFORE its producer has
-# finished (it is scheduled early and blocks in griddepcontrol.wait), so the promise does not hold for activations: measured on
-# the B200, the eager decode loop (steps queued back to back, deep chains of co-resident kernels) returned stale logits in 3 of
-# 3 runs with these loads and in 0 of 3 without (profiles/README.md, round 2).  The qualifier is therefore compiled away for
-# device code; weights stream through TMA, so nothing that matters used that path.
+# finished (it is scheduled early and blocks in griddepcontrol.wait), so the promise does not hold for activations.  The
+# qualifier is therefore compiled away for device code; weights stream through TMA, so nothing that matters used that path.
 NO_NC_LOADS = "-D__restrict__="
 FLAGS.append(NO_NC_LOADS)
 
 # Experimental builds beside the product library: libct2b200_<variant>.so, loaded through CT2B200_LIB.
 VARIANTS = {
     "restrict": None,      # keep __restrict__ (the pre-fix behaviour), for A/B timing
-    "awqtrace": ["-DCT2B200_AWQ_TRACE"],      # awq_decode.cu prints the pipeline stamps of CTA 0
 }
 
 

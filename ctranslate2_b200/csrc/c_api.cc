@@ -54,7 +54,7 @@ struct ct2b200_translator {
 extern "C" {
 
 CT2B200_API const char* ct2b200_last_error(void) { return g_error.c_str(); }
-CT2B200_API const char* ct2b200_version(void) { return "0.1.0 (sm_100a)"; }
+CT2B200_API const char* ct2b200_version(void) { return "0.1.0 (sm_90a)"; }
 CT2B200_API int64_t ct2b200_kernel_launch_count(void) { return g_kernel_launches.load(); }
 
 CT2B200_API int ct2b200_device_info(int device, int* sm_count, int* cc_major, int* cc_minor, size_t* total_mem) {
@@ -248,7 +248,7 @@ CT2B200_API int ct2b200_attention_decode(const void* qkv, void* k_cache, void* v
                              size_t workspace_bytes, int dtype, void* stream) {
   return guarded([&] {
     require_device();
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int splits = attention_decode_splits(batch, num_heads_kv, max_len, sms);
@@ -422,6 +422,13 @@ CT2B200_API int ct2b200_forward_batch(ct2b200_generator* g, const int32_t* ids, 
   return guarded([&] {
     CT2_REQUIRE(g && ids && logits, "forward_batch: null argument");
     g->impl->forward(ids, batch, time, return_log_probs != 0, logits);
+  });
+}
+
+CT2B200_API int ct2b200_bench_last_logits(ct2b200_generator* g, int64_t batch, float* logits_h, int64_t logits_len) {
+  return guarded([&] {
+    CT2_REQUIRE(g && logits_h, "null argument");
+    g->impl->bench_last_logits(batch, logits_h, logits_len);
   });
 }
 

@@ -1,4 +1,4 @@
-// common.cuh — shared device/host helpers for the sm_100a kernels of ct2b200.
+// common.cuh — shared device/host helpers for the sm_90a kernels of ct2b200.
 #pragma once
 
 #include <cuda_bf16.h>
@@ -170,7 +170,7 @@ void pdl_fence_next_launch();
 // and occupancy queries are per device, and a process may open generators on several (tag 0 = carve-out, 1 = smem limit)
 bool mark_configured(const void* kernel, int tag = 0);
 
-// All kernels of the decode step ask for the maximum shared-memory carve-out: the tcgen05 GEMMs need ~200 KB of
+// All kernels of the decode step ask for the maximum shared-memory carve-out: the wgmma GEMMs need ~200 KB of
 // shared memory per SM, and alternating between kernels with different L1/shared splits forces the SMs to drain
 // and reconfigure between launches.
 template <typename K>

@@ -185,7 +185,7 @@ class LlamaDecoder {
   int device_ = 0;
   int gemm_impl_ = CT2B200_GEMM_AUTO;
   int weight_type_ = CT2B200_WEIGHTS_STORED;
-  int sm_count_ = 148;
+  int sm_count_ = 132;
   cudaStream_t stream_ = nullptr;
   int64_t max_batch_ = 0, max_len_ = 0, chunk_rows_ = 0;
   int attn_splits_ = 1;
@@ -232,6 +232,7 @@ class Generator {
   void forward(const int32_t* ids_h, int64_t batch, int64_t time, bool log_probs, float* logits_h);
   void bench_decode(int64_t batch, int64_t prompt_len, int64_t steps, int64_t warmup, float* prefill_ms,
                     float* decode_ms, int64_t* launches);
+  void bench_last_logits(int64_t batch, float* logits_h, int64_t logits_len);
 
  private:
   void run_prefill(const int32_t* ids_d, int64_t batch, int64_t time);

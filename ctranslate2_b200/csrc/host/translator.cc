@@ -172,8 +172,8 @@ Translator::Translator(const std::string& model_dir, const ct2b200_generator_con
   CT2_CUDA_CHECK(cudaSetDevice(device_));
   int major = 0;
   CT2_CUDA_CHECK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device_));
-  if (major != 10)
-    throw std::runtime_error("ct2b200 needs an sm_100 (B200) device; found compute capability major " + std::to_string(major));
+  if (major != 9)
+    throw std::runtime_error("ct2b200 is built for sm_90a (H100); found compute capability major " + std::to_string(major));
   CT2_CUDA_CHECK(cudaDeviceGetAttribute(&sm_count_, cudaDevAttrMultiProcessorCount, device_));
   CT2_CUDA_CHECK(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
   dtype_ = cfg.compute_type;

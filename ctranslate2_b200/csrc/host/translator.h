@@ -125,7 +125,7 @@ class Translator {
 
   std::mutex mu_;                // translate / encode / bench are serialised per translator
   Seq2SeqConfig mc_;
-  int dtype_ = CT2B200_F32, device_ = 0, weight_type_ = CT2B200_WEIGHTS_STORED, sm_count_ = 148;
+  int dtype_ = CT2B200_F32, device_ = 0, weight_type_ = CT2B200_WEIGHTS_STORED, sm_count_ = 132;
   bool use_graph_ = true;
   cudaStream_t stream_ = nullptr;
 

@@ -376,7 +376,7 @@ void launch_persistent(const void* qkv, void* kc, void* vc, const float* sn, con
   const CUtensorMap tmv = tc::make_operand_map(vc, batch * Hkv * max_len, D, 2, kind, kTile);
   allow_dynamic_smem(kernel, 112 * 1024);
   static int occupancy = 0;                       // CTAs per SM: the grid must be fully co-resident (flag waits); the same on
-  if (occupancy == 0) {                           // every sm_100 device of a box
+  if (occupancy == 0) {                           // every device of a box
     int occ = 0;
     CT2_CUDA_CHECK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, kThreads, 112 * 1024));
     occupancy = std::max(1, std::min(occ, 2));
@@ -423,9 +423,9 @@ bool launch_attention_decode_persistent(const void* qkv, void* kc, void* vc, con
   }
   if (mode == 2 || dtype == CT2B200_F32 || (D != 128 && D != 64) || batch > kMaxBatch || slots < kSlots + 16) return false;
   partials += static_cast<size_t>(batch) * H * 16 * (static_cast<size_t>(D) + 2);
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
-  static int cached_dev = -1, cached_sms = 148;
+  static int cached_dev = -1, cached_sms = 132;
   if (cached_dev != dev) {
     cudaDeviceGetAttribute(&cached_sms, cudaDevAttrMultiProcessorCount, dev);
     cached_dev = dev;

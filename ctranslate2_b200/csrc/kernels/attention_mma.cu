@@ -4,7 +4,7 @@
 // cache [slot, Hkv, max_len, D]; S = Q K^T and O += P V run on mma.sync.m16n8k16 with fp32 accumulation and
 // an fp32 online softmax; P never leaves registers.  Replaces MatMul + SoftMax + MatMul over a materialised
 // [B,H,T,S] score tensor (reference src/layers/attention.cc:178-287, 536-602).
-// (Decode attention is HBM-bound and lives in attention.cu; tcgen05 needs M >= 64 rows per head-tile, which
+// (Decode attention is HBM-bound and lives in attention.cu; wgmma needs M >= 64 rows per head-tile, which
 // a 16-row warp tile does not give, so the warp-level MMA is the right instrument for this shape.)
 #include <type_traits>
 

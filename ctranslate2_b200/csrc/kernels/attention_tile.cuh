@@ -2,9 +2,8 @@
 // attention_mma.cu): cp.async staging into XOR-swizzled shared memory, S = Q K^T, online softmax, O += P V for the
 // 16 keys a warp owns.
 //
-// ncu on the first version of this loop (profiles/r01_ncu_attention_decode.md): 490 warp instructions per tile of
-// which 46 % integer address arithmetic and only 6.5 % HMMA, 5.7 cycles per issued instruction with 2 warps per
-// scheduler — issue/latency bound at 52 % of the HBM peak.  Hence everything that does not depend on the tile is
+// A naive version of this loop spends most of its instructions on integer address arithmetic and is issue bound.
+// Hence everything that does not depend on the tile is
 // hoisted: per-thread cp.async / ldmatrix offsets are computed once (the 8 rows a thread copies differ by a constant
 // stride, so the copies use immediate offsets), masking and zero-fill only exist on the ragged last tile of a
 // sequence, the accumulator rescale is skipped while the running maximum is unchanged, and the unused lower half of

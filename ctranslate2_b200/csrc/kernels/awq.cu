@@ -1,4 +1,4 @@
-// awq.cu — AWQ-INT4 (SURVEY §8 a7): ops::GemmAwq / GemvAwq / DequantizeAwq re-designed for sm_100a.
+// awq.cu — AWQ-INT4 (SURVEY §8 a7): ops::GemmAwq / GemvAwq / DequantizeAwq re-designed for sm_90a.
 //
 // Reference: src/ops/awq/gemm_gpu.cu (mma.sync m16n8k16 + split-K=8 fp16 planes + ops::Sum),
 // gemv_gpu.cu (one warp per output channel, fp32 FMA), dequantize_gpu.cu (+ cuBLAS when M >= 1024),
@@ -11,11 +11,11 @@
 // Decode GEMM (m <= 64): weight-streaming, HBM-bound.  TMA brings the packed tile [128 rows x 32 B] and the fp16
 // activation tile; four transform warps dequantize ((q - z) * s, exact subtraction then one fp16 rounding — the
 // arithmetic of the reference's dequantize_s4_to_fp16x2 + sub.f16x2 + fma.rn.f16x2) straight into the
-// 128B-swizzled K-major UMMA operand layout; tcgen05.mma.kind::f16 accumulates in TMEM (fp32); fused
+// 128B-swizzled K-major wgmma operand layout; wgmma (f16) accumulates in registers (fp32); fused
 // bias/activation/residual (or SwiGLU gate*up) epilogue.  Persistent stream-K over (tile, K-block) units like
 // gemm_tc.cu; tiles shared by several CTAs are reduced DETERMINISTICALLY (per-CTA partial slots summed in CTA
 // order by the last arriver — no float atomics).
-// Prefill (m > 64): dequantize to fp16 [N,K] scratch + the f16 tcgen05 GEMM (the reference does the same above
+// Prefill (m > 64): dequantize to fp16 [N,K] scratch + the f16 wgmma GEMM (the reference does the same above
 // M >= 1024 with cuBLAS).
 #include <algorithm>
 
@@ -110,10 +110,11 @@ __global__ void awq_dequantize_native_kernel(const int32_t* __restrict__ wp, con
 }
 
 // ---------------------------------------------------------------------------------------------
-// decode GEMM: y[m,n] = x[m,:] . deq(W)[n,:]  (swap-AB: weights on the UMMA M side)
+// decode GEMM: y[m,n] = x[m,:] . deq(W)[n,:]  (swap-AB: weights on the wgmma M side)
 // ---------------------------------------------------------------------------------------------
-constexpr int kAwqThreads = 448;      // warp 0 TMA, warp 1 MMA, warps 2-5 epilogue, warps 6-13 dequantize
-constexpr int kDeqWarps = 8;          // two threads per weight row, 32 channels (4 packed words) each
+constexpr int kAwqThreads = 288;      // warps 0-3 wgmma + epilogue, warp 4 TMA, warps 5-8 dequantize
+constexpr int kDeqWarps = 4;          // one thread per weight row, 64 channels (8 packed words) per K block
+constexpr int kRowGridBlocks = 1024;   // grid-stride element-wise kernels
 constexpr int kBKh = 64;              // fp16 elements of K per stage (one 128-byte swizzle atom)
 constexpr int kPackedTile = kTileM * kBKh / 2;      // 4096 bytes of nibbles per weight tile per stage
 
@@ -130,12 +131,13 @@ struct AwqParams {
 
 template <int BN, int NB>
 struct AwqSmem {
-  static constexpr int kA = NB * kTileM * kSwizzleBytes;      // dequantized fp16 weight tiles (UMMA M side)
+  static constexpr int kA = NB * kTileM * kSwizzleBytes;      // dequantized fp16 weight tiles (wgmma M side)
   static constexpr int kP = NB * kPackedTile;                 // packed nibbles staged by TMA
-  static constexpr int kX = BN * kSwizzleBytes;               // activations (UMMA N side)
+  static constexpr int kX = BN * kSwizzleBytes;               // activations (wgmma N side)
   static constexpr int kStage = kA + kP + kX;
-  static constexpr int kStages = (200 * 1024 / kStage) > 8 ? 8 : (200 * 1024 / kStage);
-  static constexpr size_t kBytes = static_cast<size_t>(kStages) * kStage + 1024 + 512;
+  static constexpr int kAcc = acc_bytes(NB * BN);             // accumulators parked for the epilogue
+  static constexpr int kStages = ((200 * 1024 - kAcc) / kStage) > 8 ? 8 : ((200 * 1024 - kAcc) / kStage);
+  static constexpr size_t kBytes = kAcc + static_cast<size_t>(kStages) * kStage + 1024 + 512;
 };
 
 // epilogue of one output channel over kCols batch rows; loads first, then arithmetic + stores
@@ -178,17 +180,13 @@ __global__ void __launch_bounds__(kAwqThreads, 1)
                        const __grid_constant__ CUtensorMap tm_w2, const AwqParams p) {
   using S = AwqSmem<BN, NB>;
   constexpr int kStages = S::kStages;
-  constexpr int kAccCols = BN * NB;
-  constexpr uint32_t kTmemCols = (2 * kAccCols) <= 32 ? 32 : (2 * kAccCols) <= 64 ? 64 : (2 * kAccCols) <= 128 ? 128
-                               : (2 * kAccCols) <= 256 ? 256 : 512;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + kStages * S::kStage);
+  uint32_t* accs = reinterpret_cast<uint32_t*>(smem);  // [NB * BN columns][kAccPitch]
+  uint8_t* ring = smem + S::kAcc;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(ring + kStages * S::kStage);
   uint64_t* empty_bar = full_bar + kStages;
   uint64_t* ready_bar = empty_bar + kStages;           // dequantized A tile of the stage is in place
-  uint64_t* tmem_full_bar = ready_bar + kStages;       // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;        // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
   __shared__ int s_last;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -200,31 +198,23 @@ __global__ void __launch_bounds__(kAwqThreads, 1)
   if (threadIdx.x == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(full_bar + s, 1);
-      mbar_init(empty_bar + s, 1);
+      mbar_init(empty_bar + s, 4);                     // one arrive per consumer warp
       mbar_init(ready_bar + s, kDeqWarps);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(tmem_full_bar + b, 1);
-      mbar_init(tmem_empty_bar + b, 4);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_slot, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   griddep_launch();
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ===== TMA producer: packed weight tile(s) + activation tile =====
     if (elect_one()) {
       int it = 0;
       int tile = static_cast<int>(u_begin / KB);
       int kb = static_cast<int>(u_begin - tile * KB);
       auto issue = [&](int s, int t_, int kb_, bool weights, bool acts) {
-        uint8_t* st = smem + s * S::kStage;
+        uint8_t* st = ring + s * S::kStage;
         if (weights) {
           tma_load_2d(st + S::kA, &tm_w, full_bar + s, kb_ * (kBKh / 2), t_ * kTileM, kEvictFirst);
           if (NB == 2) tma_load_2d(st + S::kA + kPackedTile, &tm_w2, full_bar + s, kb_ * (kBKh / 2), t_ * kTileM, kEvictFirst);
@@ -255,45 +245,9 @@ __global__ void __launch_bounds__(kAwqThreads, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (elect_one()) {
-      constexpr uint32_t idesc = make_idesc<1>(BN);     // kind::f16, fp16 operands, fp32 accumulate
-      int it = 0, seg = 0;
-      for (int64_t u = u_begin; u < u_end; ++seg) {
-        const int64_t tile = u / KB;
-        const int kb0 = static_cast<int>(u - tile * KB);
-        const int kb1 = static_cast<int>(min(KB, static_cast<int64_t>(kb0) + (u_end - u)));
-        const int buf = seg & 1;
-        mbar_wait(tmem_empty_bar + buf, ((seg >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t acc = tmem_base + buf * kAccCols;
-        for (int kb = kb0; kb < kb1; ++kb, ++it) {
-          const int s = it % kStages;
-          const uint32_t ph = (it / kStages) & 1;
-          mbar_wait(full_bar + s, ph);                  // activations landed
-          mbar_wait(ready_bar + s, ph);                 // weights dequantized
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + s * S::kStage);
-          const uint64_t db = make_smem_desc(sa + S::kA + S::kP);
-#pragma unroll
-          for (int w = 0; w < NB; ++w) {
-            const uint64_t da = make_smem_desc(sa + w * kTileM * kSwizzleBytes);
-#pragma unroll
-            for (int k = 0; k < kBKh / 16; ++k)
-              umma<1>(acc + w * BN, da + 2 * k, db + 2 * k, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-          }
-          umma_commit(empty_bar + s);
-        }
-        umma_commit(tmem_full_bar + buf);
-        u += kb1 - kb0;
-      }
-    }
-  } else if (warp >= 6) {
-    // ===== dequantize warps: packed nibbles -> fp16 (q - z) * s into the swizzled UMMA A tile =====
-    const int d = threadIdx.x - 192;                    // 0..255
-    const int r = d & 127;                              // tile row owned by this thread
-    const int half = d >> 7;                            // which 32-channel half of the 64-channel K block
+  } else if (warp > kProducerWarp) {
+    // ===== dequantize warps: packed nibbles -> fp16 (q - z) * s into the swizzled wgmma A tile =====
+    const int r = threadIdx.x - (kProducerWarp + 1) * 32;   // tile row owned by this thread
     const int64_t ng = p.k / p.group;
     int it = 0;
     int tile = static_cast<int>(u_begin / KB);
@@ -329,9 +283,10 @@ __global__ void __launch_bounds__(kAwqThreads, 1)
         cur_g = g;
       }
       mbar_wait(full_bar + s, ph);
-      uint8_t* st = smem + s * S::kStage;
+      uint8_t* st = ring + s * S::kStage;
 #pragma unroll
-      for (int w = 0; w < NB; ++w) {
+      for (int wh = 0; wh < 2 * NB; ++wh) {
+        const int w = wh >> 1, half = wh & 1;                 // weight, 32-channel half of the 64-channel K block
         const __half2 zb = __half2half2(__hadd(__float2half(1024.f), zc[w]));
         const __half2 zt = __half2half2(__hneg(__hadd(__float2half(64.f), zc[w])));
         const __half2 s2 = __half2half2(sc_[w]);
@@ -344,45 +299,57 @@ __global__ void __launch_bounds__(kAwqThreads, 1)
           *reinterpret_cast<uint4*>(arow + ((cc ^ (r & 7)) << 4)) = awq_dequant_word(words[c], zb, zt, s2);
         }
       }
-      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to tcgen05
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");   // generic-proxy stores -> visible to wgmma
       __syncwarp();
       if (lane == 0) mbar_arrive(ready_bar + s);
     }
   } else {
-    // ===== epilogue warps (2..5) =====
+    // ===== consumer warpgroup: wgmma over a segment's K blocks, then its epilogue =====
     griddep_wait();                                     // bias / residual may come from the previous kernel
     const int q = warp & 3;
-    const int et = threadIdx.x - 64;
+    const int et = threadIdx.x;
+    int it = 0;
     const int64_t slot_elems = static_cast<int64_t>(NB) * kTileM * BN;
-    int seg = 0;
-    for (int64_t u = u_begin; u < u_end; ++seg) {
+    for (int64_t u = u_begin; u < u_end;) {
       const int64_t tile = u / KB;
       const int kb0 = static_cast<int>(u - tile * KB);
       const int kb1 = static_cast<int>(min(KB, static_cast<int64_t>(kb0) + (u_end - u)));
       u += kb1 - kb0;
       const int64_t a0 = tile * kTileM;
-      const int buf = seg & 1;
       const bool direct = kb0 == 0 && kb1 == KB;
       float* my_slot = p.ws + (static_cast<int64_t>(blockIdx.x) * 2 + (kb0 > 0 ? 0 : 1)) * slot_elems;
-      mbar_wait(tmem_full_bar + buf, (seg >> 1) & 1);
-      tc_fence_after();
+      {
+        Acc<BN> acc[NB];
+#pragma unroll 1
+        for (int kb = kb0; kb < kb1; ++kb, ++it) {
+          const int s = it % kStages;
+          const uint32_t ph = (it / kStages) & 1;
+          mbar_wait(full_bar + s, ph);                  // activations landed
+          mbar_wait(ready_bar + s, ph);                 // weights dequantized
+          const uint32_t sa = smem_u32(ring + s * S::kStage);
+          wgmma_fence();
+#pragma unroll
+          for (int w = 0; w < NB; ++w) mma_block<1, BN>(acc[w], sa + w * kTileM * kSwizzleBytes, sa + S::kA + S::kP, kb == kb0);
+          wgmma_commit();
+          wgmma_wait();
+          if (lane == 0) mbar_arrive(empty_bar + s);
+        }
+        epi_bar_sync();                                 // the previous segment's rows have been read out of accs
+#pragma unroll
+        for (int w = 0; w < NB; ++w) acc_store<BN>(acc[w], accs + w * BN * kAccPitch);
+        epi_bar_sync();
+      }
       const int rloc = q * 32 + lane;
       const int64_t nrow = a0 + rloc;                   // output channel owned by this thread
-      const uint32_t taddr = tmem_base + buf * kAccCols + (static_cast<uint32_t>(q * 32) << 16);
 #pragma unroll 1
       for (int c0 = 0; c0 < BN; c0 += 32) {
         uint32_t rr[NB][32];
 #pragma unroll
-        for (int w = 0; w < NB; ++w) {
-          if constexpr (BN % 32 == 0) tmem_ld32(taddr + w * BN + c0, rr[w]);
-          else tmem_ld16(taddr + w * BN + c0, rr[w]);
-        }
-        if (c0 + 32 >= BN) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(tmem_empty_bar + buf);
-        }
         constexpr int kCols = (BN % 32 == 0) ? 32 : 16;
+#pragma unroll
+        for (int w = 0; w < NB; ++w)
+#pragma unroll
+          for (int j = 0; j < kCols; ++j) rr[w][j] = accs[((w * BN + c0) + j) * kAccPitch + rloc];
         if (direct) {
           float acc[NB][32];
 #pragma unroll
@@ -429,12 +396,6 @@ __global__ void __launch_bounds__(kAwqThreads, 1)
     }
   }
 
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
 }
 
 CUtensorMap make_packed_map(const void* wp, int64_t n, int64_t k) {
@@ -485,7 +446,7 @@ void awq_repack(const int32_t* qweight, const void* scales, const int32_t* qzero
   const int64_t ng = k / group;
   const int zw = layout == 2 ? static_cast<int>((group == 64 ? ((ng + 7) / 8 + 1) / 2 * 2 : (ng + 7) / 8)) : 0;
   const int sw = zw * 8;
-  awq_repack_kernel<<<148 * 8, 256, 0, st>>>(qweight, static_cast<const __half*>(scales), qzeros, layout, group, n, k, zw, sw,
+  awq_repack_kernel<<<kRowGridBlocks, 256, 0, st>>>(qweight, static_cast<const __half*>(scales), qzeros, layout, group, n, k, zw, sw,
                                              wp, static_cast<__half*>(sc), static_cast<__half*>(zr));
   check_launch();
 }
@@ -495,7 +456,7 @@ void awq_dequantize_ref_layout(const int32_t* qweight, const void* scales, const
   CT2_REQUIRE(layout == 1 || layout == 2, "awq: layout must be 1 (AWQ_GEMM) or 2 (AWQ_GEMV)");
   const int64_t ng = k / group;
   const int zw = layout == 2 ? static_cast<int>((group == 64 ? ((ng + 7) / 8 + 1) / 2 * 2 : (ng + 7) / 8)) : 0;
-  awq_dequantize_ref_layout_kernel<<<148 * 8, 256, 0, st>>>(qweight, static_cast<const __half*>(scales), qzeros, layout, group,
+  awq_dequantize_ref_layout_kernel<<<kRowGridBlocks, 256, 0, st>>>(qweight, static_cast<const __half*>(scales), qzeros, layout, group,
                                                             n, k, zw, zw * 8, static_cast<__half*>(w_out));
   check_launch();
 }
@@ -512,13 +473,13 @@ __global__ void awq_group_major_kernel(const __half* __restrict__ sc, const __ha
 }  // namespace
 
 void awq_build_group_major(const AwqNative& w, void* sz_out, cudaStream_t st) {
-  awq_group_major_kernel<<<148 * 4, 256, 0, st>>>(static_cast<const __half*>(w.sc), static_cast<const __half*>(w.zr), w.n,
+  awq_group_major_kernel<<<kRowGridBlocks, 256, 0, st>>>(static_cast<const __half*>(w.sc), static_cast<const __half*>(w.zr), w.n,
                                                   w.k / w.group, static_cast<__half2*>(sz_out));
   check_launch();
 }
 
 void awq_dequantize_native(const AwqNative& w, void* w_out /* f16 [n,k] */, cudaStream_t st) {
-  awq_dequantize_native_kernel<<<148 * 8, 256, 0, st>>>(static_cast<const int32_t*>(w.wp), static_cast<const __half*>(w.sc),
+  awq_dequantize_native_kernel<<<kRowGridBlocks, 256, 0, st>>>(static_cast<const int32_t*>(w.wp), static_cast<const __half*>(w.sc),
                                                         static_cast<const __half*>(w.zr), w.group, w.n, w.k,
                                                         static_cast<__half*>(w_out));
   check_launch();

@@ -1,25 +1,21 @@
-// awq_decode.cu — AWQ-INT4 weight-streaming GEMM of the decode step (m <= 64) on tcgen05, A operand in TENSOR MEMORY.
+// awq_decode.cu — AWQ-INT4 weight-streaming GEMM of the decode step (m <= 64) on wgmma, A operand in REGISTERS.
 //
 // Replaces ops::GemmAwq / ops::GemvAwq (+ ops::Sum over split-K planes, + bias / activation / Mul) of the reference
 // (src/ops/awq/gemm_gpu.cu, gemv_gpu.cu; dispatch src/layers/common.cc:402-438) by one kernel per Dense.
 //
-// Same plan as gemm_decode.cu (one tile per CTA, "swap AB": 128 output channels = the UMMA M side, activations = N side;
+// Same plan as gemm_decode.cu (one tile per CTA, "swap AB": 128 output channels = the wgmma M side, activations = N side;
 // DSMEM split-K cluster chosen so that tiles x CS fills the SMs in one wave; weights prefetched before griddepcontrol.wait),
 // plus what 4-bit weights need:
 //   * the only bytes that come from HBM are the packed nibbles.  A ring slot holds a SUPER-BLOCK of four K blocks (256 input
-//     channels): per weight one TMA box of 128 rows x 128 bytes (SWIZZLE_128B, so that the 32 rows a warp reads land in
+//     channels): per weight one TMA box of 128 rows x 128 bytes (SWIZZLE_128B, so that the rows a warp reads land in
 //     different banks), the {scale, zero} pairs of its groups (512 B each, cp.async.bulk from the group-major array) and the
-//     four activation atoms, so the transform warps never touch global memory.  The box width matters: TMA works row by row,
-//     and with one box per 64-channel block (128 rows x 32 bytes — the first version of this kernel) the row requests, not the
-//     bytes, set the pace: ncu showed every transform warp parked on the "slot full" barrier, 10 GB/s per SM and DRAM at 7-16 %.
-//     (Before that, round 1 fetched the pairs with per-thread global loads inside the loop: 64 % long_scoreboard.)
-//   * the dequantized fp16 operand never goes back to shared memory.  int4 -> fp16 at HBM speed is 5.8 TB/s of nibbles =
-//     23 TB/s of fp16, i.e. 82 B/clk/SM written + 82 B/clk/SM read by the tensor core: more than the 128 B/clk of the shared
-//     memory port.  Instead the thread that owns output channel r converts the 64 channels of its row in registers
+//     four activation atoms, so the consumer warps never touch global memory.  TMA works row by row: one wide box per
+//     super-block needs a quarter of the row requests of one box per 64-channel block.
+//   * the dequantized fp16 operand never goes back to shared memory: wgmma takes its A operand from registers.  The thread
+//     that holds rows g, g + 8 and the channel pairs 2t, 2t + 1 (+ 8) of the m64k16 A fragment converts exactly those pairs
 //     ((q - z) * s: exact subtraction, one fp16 rounding — the arithmetic of the reference's dequantize_s4_to_fp16x2 +
-//     sub.f16x2 + fma.rn.f16x2) and writes them with ONE tcgen05.st.32x32b.x32 into TMEM lane r, columns [32 x stage): the
-//     K-major A layout tcgen05.mma reads directly (cute::UMMA::tmem_frg, M = 128: lane = row, two fp16 per 32-bit column).
-//   * tcgen05.mma.kind::f16 with A from TMEM, B (activations) from 128B-swizzled smem, fp32 accumulators in TMEM;
+//     sub.f16x2 + fma.rn.f16x2): in the native word layout the pair (k 2t, k 2t + 1) of a word is one lop3 away.
+//   * wgmma f16 with A from registers, B (activations) from 128B-swizzled smem, fp32 accumulators in registers;
 //     epilogue = gemm_decode_common.cuh (float arm).
 #include <map>
 #include <mutex>
@@ -35,27 +31,13 @@ namespace {
 using namespace tc;
 using namespace dec;
 
-constexpr int kThreads = 704;          // warp 0 TMA, warp 1 MMA, warps 2-5 epilogue, warps 6-21 transform
-constexpr int kDeqWarps = 16;          // 4 transform groups of 4 warps; group g owns the K blocks it % 4 == g, so four
-constexpr int kGroups = 4;             // blocks are converted CONCURRENTLY (LDS -> lop3/hfma -> tcgen05.st is a latency chain)
-constexpr int kGroupWarps = kDeqWarps / kGroups;
+constexpr int kThreads = kTcThreads;   // warps 0-3 convert + wgmma + epilogue, warp 4 TMA
 constexpr int kBKh = 64;               // fp16 channels per K block (one 128-byte swizzle atom of the activation operand)
-constexpr int kSub = 4;                         // K blocks per ring slot = transform groups: group g converts sub-block g
+constexpr int kSub = 4;                         // K blocks per ring slot
 constexpr int kSlotK = kSub * kBKh;             // 256 input channels per slot
 constexpr int kPacked = kTileM * kSlotK / 2;    // 16 KB of nibbles per weight per slot (128 rows x 128 B, SWIZZLE_128B)
 constexpr int kPairBytes = 512;                 // the 128 {scale, zero} pairs of one group of a weight
 constexpr int kPairs = kSub * kPairBytes;       // up to 4 groups per slot (group 64); 2 KB keeps what follows 1024-byte aligned
-constexpr int kAColsPerBlock = kBKh / 2;        // 32 TMEM columns hold the 64 fp16 channels of a block
-// TMEM: TWO accumulator sets (one per MMA issuer: a single thread issuing the 8-32 small MMAs of a slot, with their barrier
-// waits and commits, was the pace-setter of the kernel — 1 700 of 2 400 cycles per slot in the stamp trace) in columns
-// [0, 2 * NB * BN), dequantized A stages above.  Block `it` uses A stage it % kAStages.
-constexpr int kIssuers = 2;
-template <int BN, int NB> struct AStages {
-  static constexpr int acc_cols = kIssuers * NB * BN;
-  static constexpr int raw = (512 - acc_cols) / (NB * kAColsPerBlock);
-  static constexpr int value = raw > 12 ? 12 : raw;             // 14 -> 12 | 7 / 6 / 4 (NB = 2, BN = 16 / 32 / 64)
-};
-constexpr int kMaxAStages = 12;
 constexpr int kMaxP = 8;
 
 struct AwqDecParams {
@@ -72,47 +54,27 @@ struct AwqDecSmem {
   static constexpr int kAct = BN * kSwizzleBytes;                           // one activation atom (64 channels)
   static constexpr int kP = NB * (kPacked + kPairs) + kSub * kAct;          // one ring slot: nibbles | pairs | 4 activation atoms
   static constexpr int kCtrl = 1024;
+  static constexpr int kAcc = acc_bytes(NB * BN);                           // accumulators parked for the row-per-thread epilogue
   static size_t red_bytes(int cs) { return cs > 1 ? static_cast<size_t>(cs) * NB * (BN / 16) * ((16 + cs - 1) / cs) * kTileM * 4 : 0; }
   static size_t bytes(int p_stages, int cs) {
-    return static_cast<size_t>(p_stages) * kP + kCtrl + red_bytes(cs) + 1024;
+    return kAcc + static_cast<size_t>(p_stages) * kP + kCtrl + red_bytes(cs) + 1024;
   }
 };
 
-// D[tmem] (+)= A[tmem] * B[smem descriptor]
-__device__ __forceinline__ void umma_ts_f16(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n}\n"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate));
+// channels (2t, 2t + 1) of a native word: pair t is the bottom (t even) or top (t odd) nibble pair of w >> (t >= 2 ? 8 : 0);
+// mask / mul / add select the arm of awq_dequant_word (bottom: h - (1024 + z); top: h / 16 - (64 + z)), then one rounding by s
+__device__ __forceinline__ uint32_t awq_dequant_pair(uint32_t w, uint32_t shift, uint32_t mask, __half2 mul, __half2 add, __half2 s2) {
+  constexpr uint32_t kLut = (0xf0 & 0xcc) | 0xaa, kMagic = 0x64006400;
+  uint32_t h;
+  asm volatile("lop3.b32 %0, %1, %2, %3, %4;" : "=r"(h) : "r"(w >> shift), "r"(mask), "n"(kMagic), "n"(kLut));
+  const __half2 v = __hmul2(__hfma2(*reinterpret_cast<__half2*>(&h), mul, add), s2);
+  return *reinterpret_cast<const uint32_t*>(&v);
 }
-// 32 lanes x 32 columns: thread t of the warp writes r[0..31] to its lane, columns taddr.col + [0, 32)
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-      "{%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-      "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-        "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-        "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-        "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
 // global -> shared bulk copy (bytes % 16 == 0, both addresses 16-byte aligned), completion on an mbarrier
 __device__ __forceinline__ void bulk_load(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
                ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
 }
-
-// -DCT2B200_AWQ_TRACE (python -m ctranslate2_b200.build --variant awqtrace): CTA 0 records SM cycle stamps of the pipeline
-// events of its first 16 super-blocks and prints them when it is done.  Not compiled into the product library.
-#ifdef CT2B200_AWQ_TRACE
-#define AWQ_TRACE_DECL __shared__ long long s_trace[16][12];
-#define AWQ_TRACE(sb, slot) do { if (blockIdx.x == 0 && (sb) < 16) s_trace[sb][slot] = clock64(); } while (0)
-#else
-#define AWQ_TRACE_DECL
-#define AWQ_TRACE(sb, slot) do { } while (0)
-#endif
 
 template <int BN, int NB, int CS>
 __global__ void __launch_bounds__(kThreads, 1)
@@ -121,25 +83,17 @@ __global__ void __launch_bounds__(kThreads, 1)
   using S = AwqDecSmem<BN, NB>;
   using T = __half;
   const DecParams& p = ap.d;
-  constexpr uint32_t kTmemCols = 512;
   constexpr int cp16 = (16 + CS - 1) / CS;
   constexpr int cpr = (BN / 16) * cp16;
-  constexpr int kAStages = AStages<BN, NB>::value;
-  constexpr int kAccCols = AStages<BN, NB>::acc_cols;      // accumulator set i at columns [i * NB * BN, +NB * BN)
-  static_assert(kAStages >= kSub, "every transform group needs an A stage");
 
   extern __shared__ uint8_t smem_raw[];
-  AWQ_TRACE_DECL
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* p_ring = smem;                                         // [p_stages][nibbles NB x 4 KB | pairs NB x 512 B | x BN x 128 B]
+  uint32_t* accs = reinterpret_cast<uint32_t*>(smem);             // [NB * BN columns][kAccPitch]
+  uint8_t* p_ring = smem + S::kAcc;                               // [p_stages][nibbles NB x 16 KB | pairs NB x 2 KB | x 4 x BN x 128 B]
   const int PD = ap.p_stages;
   uint8_t* ctrl = p_ring + static_cast<size_t>(PD) * S::kP;
   uint64_t* p_full = reinterpret_cast<uint64_t*>(ctrl);           // [kMaxP] TMA landed
-  uint64_t* p_free = p_full + kMaxP;                              // [kMaxP] transform warps + the MMA commit
-  uint64_t* a_ready = p_free + kMaxP;                             // [kAStages] A stage written to TMEM (the group's warps)
-  uint64_t* a_free = a_ready + kMaxAStages;                       // [kAStages] MMAs that read it retired
-  uint64_t* acc_bar = a_free + kMaxAStages;
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_bar + 1);
+  uint64_t* p_free = p_full + kMaxP;                              // [kMaxP] the consumer warps are done with the slot
   uint32_t* red = reinterpret_cast<uint32_t*>(ctrl + S::kCtrl);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -153,58 +107,16 @@ __global__ void __launch_bounds__(kThreads, 1)
   if (threadIdx.x == 0) {
     for (int s = 0; s < PD; ++s) {
       mbar_init(p_full + s, 1);
-      mbar_init(p_free + s, kDeqWarps + kIssuers);
+      mbar_init(p_free + s, 4);                                    // one arrive per consumer warp
     }
-    for (int s = 0; s < kAStages; ++s) {
-      mbar_init(a_ready + s, kGroupWarps);
-      mbar_init(a_free + s, 1);
-    }
-    mbar_init(acc_bar, kIssuers);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_slot, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   griddep_launch();
   if (CS > 1) cluster_arrive();
 
-  // ===== MMA issuer `half` (warp 1: 0, warp 2: 1): sub-blocks 2 half, 2 half + 1 of every slot into accumulator set `half` =====
-  auto mma_issuer = [&](int half) {
-    constexpr uint32_t idesc = make_idesc<1>(BN);
-    const uint32_t acc = tmem_base + half * (NB * BN);
-#pragma unroll 1
-    for (int sb = 0; sb < nsb; ++sb) {
-      const int sp = sb % PD;
-      mbar_wait(p_full + sp, (sb / PD) & 1);                    // activations of this super-block landed
-      if (half == 0) AWQ_TRACE(sb, 1);
-      const uint32_t act0 = smem_u32(p_ring + static_cast<size_t>(sp) * S::kP + NB * (kPacked + kPairs));
-#pragma unroll 1
-      for (int jj = 0; jj < kSub / kIssuers; ++jj) {
-        const int j = half * (kSub / kIssuers) + jj;
-        const int it = sb * kSub + j, sa = it % kAStages;
-        mbar_wait(a_ready + sa, (it / kAStages) & 1);           // weights dequantized into TMEM
-        if (half == 0 && jj == 0) AWQ_TRACE(sb, 2);
-        if (half == 0 && jj == 1) AWQ_TRACE(sb, 3);
-        tc_fence_after();
-        const uint32_t ta = tmem_base + kAccCols + sa * (NB * kAColsPerBlock);
-        const uint64_t db = make_smem_desc(act0 + j * S::kAct);
-#pragma unroll
-        for (int w = 0; w < NB; ++w)
-#pragma unroll
-          for (int k = 0; k < kBKh / 16; ++k)                   // K = 16 per instruction = 8 TMEM columns of A
-            umma_ts_f16(acc + w * BN, ta + w * kAColsPerBlock + k * 8, db + 2 * k, idesc, (sb > 0 || jj > 0 || k > 0) ? 1u : 0u);
-        umma_commit(a_free + sa);
-      }
-      umma_commit(p_free + sp);
-      if (half == 0) AWQ_TRACE(sb, 4);
-    }
-    umma_commit(acc_bar);
-  };
-
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ===== TMA producer: packed nibbles, {scale, zero} pairs (both weights are constants: issued before the grid
     // dependency resolves) and the activation block =====
     if (elect_one()) {
@@ -229,7 +141,6 @@ __global__ void __launch_bounds__(kThreads, 1)
       const int pre = min(PD, nsb);
 #pragma unroll 1
       for (int i = 0; i < pre; ++i) {
-        AWQ_TRACE(i, 0);
         mbar_expect_tx(p_full + i, tx);
         weights(i, sb_lo + i);
       }
@@ -240,102 +151,76 @@ __global__ void __launch_bounds__(kThreads, 1)
       for (int it = pre; it < nsb; ++it) {
         const int s = it % PD;
         mbar_wait(p_free + s, ((it / PD) & 1) ^ 1);
-        AWQ_TRACE(it, 0);
         mbar_expect_tx(p_full + s, tx);
         weights(s, sb_lo + it);
         acts(s, sb_lo + it);
       }
     }
-  } else if (warp == 1) {
-    if (elect_one()) mma_issuer(0);
-  } else if (warp >= 6) {
-    // ===== transform warps: nibbles -> fp16 (q - z) * s, registers -> TMEM =====
-    // thread -> (transform group, tile row).  A warp may only touch TMEM lanes [32 * (warp % 4), +32): the row quadrant of a
-    // warp is warp % 4 (any bijection inside the group of four consecutive warps works).
-    const int grp = (warp - 6) >> 2;
-    const int quad = warp & 3;
-    const int r = quad * 32 + lane;
-    const uint32_t lane_base = static_cast<uint32_t>(quad * 32) << 16;
-    // group grp converts sub-block grp of every super-block; its 32 bytes of row r are the 16-byte chunks 2 grp, 2 grp + 1
-    // of the row's 128 bytes, stored at chunk ^ (r % 8) by the 128-byte swizzle
-    const int pair_slot = (grp * kBKh) / ap.group < ngs ? (grp * kBKh) / ap.group : ngs - 1;
-    const uint32_t ch0 = static_cast<uint32_t>((2 * grp) ^ (r & 7)) * 16u, ch1 = static_cast<uint32_t>((2 * grp + 1) ^ (r & 7)) * 16u;
-#pragma unroll 1
-    for (int sb = 0; sb < nsb; ++sb) {
-      const int it = sb * kSub + grp;
-      const int sp = sb % PD, sa = it % kAStages;
-      mbar_wait(p_full + sp, (sb / PD) & 1);
-      if (threadIdx.x == 6 * 32) AWQ_TRACE(sb, 5);
-      if (threadIdx.x == 18 * 32) AWQ_TRACE(sb, 9);
-      const uint8_t* pk = p_ring + static_cast<size_t>(sp) * S::kP;
-      const uint32_t ta = tmem_base + lane_base + kAccCols + sa * (NB * kAColsPerBlock);
-#pragma unroll
-      for (int w = 0; w < NB; ++w) {
-        uint32_t v[32];
-        const __half2 sz = *reinterpret_cast<const __half2*>(pk + NB * kPacked + w * kPairs + pair_slot * kPairBytes + r * 4);
-        const __half sc = __low2half(sz), zp = __high2half(sz);
-        const __half2 zb = __half2half2(__hadd(__float2half(1024.f), zp));
-        const __half2 zt = __half2half2(__hneg(__hadd(__float2half(64.f), zp)));
-        const __half2 s2 = __half2half2(sc);
-        const uint8_t* row = pk + w * kPacked + r * kSwizzleBytes;
-        const uint4 w0 = *reinterpret_cast<const uint4*>(row + ch0);
-        const uint4 w1 = *reinterpret_cast<const uint4*>(row + ch1);
-        const uint32_t words[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {                  // word c = channels 8c .. 8c+7 = TMEM columns 4c .. 4c+3
-          const uint4 d = awq_dequant_word(words[c], zb, zt, s2);
-          v[4 * c + 0] = d.x;
-          v[4 * c + 1] = d.y;
-          v[4 * c + 2] = d.z;
-          v[4 * c + 3] = d.w;
-        }
-        // the A stage is free once the MMAs of block it - kAStages have retired (waited for AFTER the first conversion)
-        if (w == 0) {
-          if (threadIdx.x == 6 * 32) AWQ_TRACE(sb, 6);
-          if (it >= kAStages) {
-            mbar_wait(a_free + sa, ((it / kAStages) & 1) ^ 1);
-            tc_fence_after();
-          }
-          if (threadIdx.x == 6 * 32) AWQ_TRACE(sb, 7);
-        }
-        tmem_st32(ta + w * kAColsPerBlock, v);
-      }
-      tmem_st_wait();
-      if (threadIdx.x == 6 * 32) AWQ_TRACE(sb, 8);
-      if (threadIdx.x == 18 * 32) AWQ_TRACE(sb, 10);
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(a_ready + sa);
-        mbar_arrive(p_free + sp);
-      }
-    }
   } else {
-    // ===== epilogue warps (2..5): thread = output channel =====
+    // ===== consumer warpgroup: nibbles -> fp16 A fragments in registers -> wgmma; then thread = output channel =====
     const int q = warp & 3;
     const int rloc = q * 32 + lane;
     const int64_t arow = static_cast<int64_t>(a0) + rloc;
     const bool row_ok = rloc < p.tile_rows && arow < p.n;
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-    if (warp == 2) {                                   // the second MMA issuer lives in an epilogue warp (idle until the end)
-      if (elect_one()) mma_issuer(1);
-      __syncwarp();
+    {
+      const int t = lane & 3;                                      // channel pair of the A fragment held by this thread
+      const uint32_t shift = (t & 2) ? 8u : 0u, mask = (t & 1) ? 0x00f000f0u : 0x000f000fu;
+      const __half2 mul = __float2half2_rn((t & 1) ? 0.0625f : 1.f);
+      Acc<BN> acc[NB];
+#pragma unroll 1
+      for (int sb = 0; sb < nsb; ++sb) {
+        const int sp = sb % PD;
+        mbar_wait(p_full + sp, (sb / PD) & 1);
+        const uint8_t* pk = p_ring + static_cast<size_t>(sp) * S::kP;
+        const uint32_t act0 = smem_u32(pk + NB * (kPacked + kPairs));
+#pragma unroll 1
+        for (int j = 0; j < kSub; ++j) {                           // K block j of the slot: 32 bytes of every packed row
+          const int pair_slot = (j * kBKh) / ap.group < ngs ? (j * kBKh) / ap.group : ngs - 1;
+          const uint64_t db = make_smem_desc(act0 + j * S::kAct);
+#pragma unroll
+          for (int w = 0; w < NB; ++w)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              uint32_t a[kBKh / 16][4];
+#pragma unroll
+              for (int rr = 0; rr < 2; ++rr) {                     // rows g, g + 8 of this warp's 16
+                const int r = h * 64 + q * 16 + (lane >> 2) + rr * 8;
+                const __half2 sz = *reinterpret_cast<const __half2*>(pk + NB * kPacked + w * kPairs + pair_slot * kPairBytes + r * 4);
+                const __half zp = __high2half(sz);
+                const __half2 add = __half2half2((t & 1) ? __hneg(__hadd(__float2half(64.f), zp)) : __hneg(__hadd(__float2half(1024.f), zp)));
+                const __half2 s2 = __half2half2(__low2half(sz));
+                // the 16-byte chunks 2j, 2j + 1 of the row's 128 bytes are stored at chunk ^ (r % 8) by the 128-byte swizzle
+                const uint8_t* row = pk + w * kPacked + r * kSwizzleBytes;
+                const uint4 w0 = *reinterpret_cast<const uint4*>(row + (((2 * j) ^ (r & 7)) << 4));
+                const uint4 w1 = *reinterpret_cast<const uint4*>(row + (((2 * j + 1) ^ (r & 7)) << 4));
+                const uint32_t words[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+#pragma unroll
+                for (int k = 0; k < kBKh / 16; ++k) {              // word 2k = channels 16k .. 16k+7, word 2k+1 = 16k+8 .. 16k+15
+                  a[k][rr] = awq_dequant_pair(words[2 * k], shift, mask, mul, add, s2);
+                  a[k][2 + rr] = awq_dequant_pair(words[2 * k + 1], shift, mask, mul, add, s2);
+                }
+              }
+              wgmma_fence();
+#pragma unroll
+              for (int k = 0; k < kBKh / 16; ++k)
+                wgmma_rs_f16(acc[w].d[h][0], a[k], db + 2 * k, (sb == 0 && j == 0 && k == 0) ? 0u : 1u);
+              wgmma_commit();
+              wgmma_wait();                                        // the A registers are rewritten by the next conversion
+            }
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(p_free + sp);
+      }
+#pragma unroll
+      for (int w = 0; w < NB; ++w) acc_store<BN>(acc[w], accs + w * BN * kAccPitch);
+      epi_bar_sync();
     }
     griddep_wait();
     float bias_t = 0.f;
     if (row_ok && p.bias) bias_t = to_f32(static_cast<const T*>(p.bias)[arow]);
-    mbar_wait(acc_bar, 0);
-    tc_fence_after();
-    // the two accumulator sets are partial sums over alternate halves of every slot
     auto load_acc = [&](int c0, uint32_t (&r)[NB][16]) {
 #pragma unroll
-      for (int w = 0; w < NB; ++w) {
-        uint32_t r1[16];
-        tmem_ld16x16(taddr + w * BN + c0, r[w]);
-        tmem_ld16x16(taddr + NB * BN + w * BN + c0, r1);
-#pragma unroll
-        for (int j = 0; j < 16; ++j) r[w][j] = __float_as_uint(__uint_as_float(r[w][j]) + __uint_as_float(r1[j]));
-      }
+      for (int w = 0; w < NB; ++w) acc_load<16>(accs + (w * BN + c0) * kAccPitch, rloc, r[w]);
     };
     if constexpr (CS == 1) {
 #pragma unroll 1
@@ -370,10 +255,10 @@ __global__ void __launch_bounds__(kThreads, 1)
 
   if constexpr (CS > 1) {
     __syncwarp();
-    if (warp < 2 || warp >= 6) cluster_wait();         // phase 1 (the epilogue warps consumed it above)
+    if (warp == kProducerWarp) cluster_wait();         // phase 1 (the consumer warps consumed it above)
     cluster_arrive();
     cluster_wait();
-    if (warp >= 2 && warp < 6) {
+    if (warp < kProducerWarp) {
       const int q = warp & 3;
       const int rloc = q * 32 + lane;
       const int64_t arow = static_cast<int64_t>(a0) + rloc;
@@ -400,24 +285,6 @@ __global__ void __launch_bounds__(kThreads, 1)
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-#ifdef CT2B200_AWQ_TRACE
-  if (blockIdx.x == 0 && threadIdx.x == 0) {
-    const long long t0 = s_trace[0][0];
-    printf("awq trace BN=%d NB=%d CS=%d PD=%d nsb=%d: per super-block [tma issue | mma: acts landed, a_ready(0), a_ready(3), commit | "
-           "group0: slot full, converted, a_free, st done | group3: slot full, st done] cycles since the first issue\n",
-           BN, NB, CS, PD, nsb);
-    for (int sb = 0; sb < min(nsb, 16); ++sb)
-      printf("  sb %2d: %6lld | %6lld %6lld %6lld %6lld | %6lld %6lld %6lld %6lld | %6lld %6lld\n", sb, s_trace[sb][0] - t0,
-             s_trace[sb][1] - t0, s_trace[sb][2] - t0, s_trace[sb][3] - t0, s_trace[sb][4] - t0, s_trace[sb][5] - t0,
-             s_trace[sb][6] - t0, s_trace[sb][7] - t0, s_trace[sb][8] - t0, s_trace[sb][9] - t0, s_trace[sb][10] - t0);
-  }
-#endif
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
 }
 
 // ---- host side ----
@@ -442,12 +309,8 @@ CUtensorMap make_packed_map(const void* wp, int64_t n, int64_t k, int box_rows) 
 template <int BN, int NB>
 int p_stages_for(int cs, int nkb) {
   using S = AwqDecSmem<BN, NB>;
-#ifdef CT2B200_AWQ_TRACE
-  const size_t cap = 212 * 1024;          // room for the static trace buffer
-#else
   const size_t cap = 220 * 1024;
-#endif
-  const size_t fixed = S::kCtrl + S::red_bytes(cs) + 1024;
+  const size_t fixed = S::kAcc + S::kCtrl + S::red_bytes(cs) + 1024;
   if (fixed + 2 * S::kP > cap) return 0;
   int st = static_cast<int>((cap - fixed) / S::kP);
   st = std::min(st, kMaxP);
@@ -456,11 +319,7 @@ int p_stages_for(int cs, int nkb) {
 
 template <int BN, int NB, int CS>
 void configure_once() {
-#ifdef CT2B200_AWQ_TRACE
-  allow_dynamic_smem(awq_decode_kernel<BN, NB, CS>, 222 * 1024);
-#else
   allow_dynamic_smem(awq_decode_kernel<BN, NB, CS>, 226 * 1024);
-#endif
 }
 
 template <int BN, int NB, int CS>
@@ -507,10 +366,9 @@ AwqPlan plan_awq(int64_t n, int kb_total /* super-blocks */, int sm_count) {
       case 3: maxc = clusters_for<BN, NB, 3>(ps, sm_count); break;
       default: maxc = clusters_for<BN, NB, 4>(ps, sm_count); break;
     }
-    // Tile height.  The transform converts all 128 rows of a block whatever the tile height, so full-height tiles waste nothing;
-    // but since the kernel waits on the HBM stream rather than on the conversion (stamp trace, profiles/README.md), a shorter
-    // tile that puts the stream on more SMs wins when 128-row tiles leave many idle: gate/up of Llama-3-8B is 112 tiles of 128
-    // rows on 148 SMs, 138 tiles of 104.  cost = streamed rows x K blocks per CTA (+ the cluster exchange).
+    // Tile height.  The conversion covers all 128 rows of a block whatever the tile height, so full-height tiles waste nothing;
+    // a shorter tile that puts the stream on more SMs wins when 128-row tiles leave many idle.
+    // cost = streamed rows x K blocks per CTA (+ the cluster exchange).
     const int full = static_cast<int>((n + 127) / 128);
     int cand[2] = {128, 128};
     if (!force_rows && full * 10 < maxc * 9) {
@@ -602,10 +460,8 @@ bool run_m(const void* x, const AwqNative& w, const AwqNative* w2, int64_t m, co
   return run<64, NB>(x, w, w2, m, p, st);
 }
 
-// CT2B200_AWQ_DECODE=0 falls back to the general stream-K kernel of awq.cu (CT2B200_AWQ_DECODE_GLU does the same for the
-// fused gate/up launch only).  Measured in the decode graph of a Llama-3-8B AWQ model (tools/decode_once.py, B200): with the
-// four concurrent transform groups this kernel takes 3.93 ms / step at bsz 1 and 4.84 ms at bsz 32, the general kernel
-// 4.04 / 6.0 ms.  Both are bound by the int4 -> fp16 transform (~1 TB/s of packed weights), not by HBM.
+// CT2B200_AWQ_DECODE=0 selects the general stream-K kernel of awq.cu (CT2B200_AWQ_DECODE_GLU does the same for the
+// fused gate/up launch only).
 bool enabled() { return env_int("CT2B200_AWQ_DECODE", CT2B200_DEFAULT_AWQ_DECODE) != 0; }
 bool glu_enabled() { return env_int("CT2B200_AWQ_DECODE_GLU", env_int("CT2B200_AWQ_DECODE", CT2B200_DEFAULT_AWQ_DECODE)) != 0; }
 

@@ -13,8 +13,7 @@
 //
 // Native layout (ct2b200_awq_repack): wp int32 [n, k/8] (word w of row c = channels 8w .. 8w+7 in nibbles {0,4,1,5,2,6,3,7}),
 // sc / zr fp16 [n, k/group].  group = 128 (what AutoAWQ writes and the reference's kernels assume), k % 128 == 0, k <= 16384;
-// other shapes and m > 1 go to the tensor-core kernels (awq_decode.cu, awq.cu; at m = 2 they are already faster: 3.80 vs 4.69 ms
-// per 8B decode step on the B200).
+// other shapes and m > 1 go to the tensor-core kernels (awq_decode.cu, awq.cu).
 #include "awq_common.cuh"
 #include "gemm_decode_common.cuh"
 #include "kernels.h"
@@ -43,7 +42,7 @@ struct GemvParams {
 // One warp = R output channels (of each of the NB weights).  A "trip" is 1024 input channels: a lane owns 32 of them = one
 // 16-byte load of nibbles per channel and 64 bytes of the activation row, which are converted once and reused by all NB * R
 // channels — with one channel per warp the activation reads through L1 (8 KB per 2 KB of nibbles at k = 4096) cost as many
-// load wavefronts as the HBM stream itself (measured: 1.6 TB/s).  Two trips of all channels are requested before the first is
+// load wavefronts as the HBM stream itself.  Two trips of all channels are requested before the first is
 // used (128 bytes per lane in flight).  The group scales / zeros of a row (k / 128 of each) are fetched once with coalesced
 // loads — lane g holds group g + 32 c — and handed to the lane that needs them by shuffle: trip t uses group 8 t + lane / 4.
 constexpr int kMaxQuads = 4;           // quads of 4 trips: k <= 16384
@@ -178,10 +177,8 @@ void launch_gemv(const void* x, const AwqNative& a, const AwqNative* b, const Ge
   const GemvWeight w1 = b ? GemvWeight{static_cast<const uint32_t*>(b->wp), static_cast<const __half*>(b->sc),
                                        static_cast<const __half*>(b->zr)} : w0;
   const int64_t groups = (a.n + R - 1) / R;        // row groups = warps at KS = 1
-  // (a variant whose register copy of the scales is sized for k <= 4096 — 103 instead of 128 registers — measured SLOWER: 2.94 vs
-  // 2.69 ms per 8B decode step; the occupancy is 2 CTAs per SM either way)
   const int force_ks = dec::env_int("CT2B200_AWQ_GEMV_KS", 0);
-  const bool split = force_ks ? force_ks == 2 : (groups < 2 * 148 * kWarps && a.k >= 4096);
+  const bool split = force_ks ? force_ks == 2 : (groups < 2 * static_cast<int64_t>(dec::sm_count_of_current_device()) * kWarps && a.k >= 4096);
   const dim3 block(kWarps * 32);
   if (split) {
     const dim3 grid(static_cast<unsigned>((groups * 2 + kWarps - 1) / kWarps));
@@ -198,7 +195,7 @@ bool covered(const AwqNative& w, int64_t m, const void* x) {
          (reinterpret_cast<uintptr_t>(x) & 15) == 0 && (reinterpret_cast<uintptr_t>(w.wp) & 15) == 0;
 }
 
-// CT2B200_AWQ_GEMV: 1 = use this kernel for m == 1 (opt-in until its hardware validation is recorded in profiles/README.md)
+// CT2B200_AWQ_GEMV: 1 = use this kernel for m == 1
 bool enabled() { return dec::env_int("CT2B200_AWQ_GEMV", CT2B200_DEFAULT_AWQ_GEMV) != 0; }
 
 }  // namespace

@@ -67,7 +67,7 @@ struct SplitKWorkspace {
   int32_t* accum2 = nullptr;        // fully-overwritten partial slots of the float (f16/AWQ) kernels: never needs zeroing
   size_t accum_elems = 0;
   size_t num_counters = 0;
-  int sm_count = 148;
+  int sm_count = 132;
 
   static constexpr size_t kAccumElems = size_t(16) << 20;  // 64 MiB of int32
   static constexpr size_t kCounters = 1 << 16;

@@ -1,22 +1,22 @@
-// gemm_decode.cu — weight-streaming GEMM of the decode step (m <= 64 activation rows) on tcgen05.
+// gemm_decode.cu — weight-streaming GEMM of the decode step (m <= 64 activation rows) on wgmma.
 //
 // Replaces, for the Dense layers of one decode step, the reference chain
 //   ops::Gemm (cuBLAS IMMA, int32 C in HBM) -> ops::Dequantize::dequantize_gemm_output -> ops::Add / ops::Mul
 // (reference src/layers/common.cc:353-401, src/ops/gemm.cc:45-107, src/ops/dequantize_gpu.cu:30-144) by ONE kernel.
 //
 // Shape of the problem: y[m, n] = x[m, k] * W[n, k]^T with m <= 64: every weight byte is used once, so the kernel is a
-// pure HBM stream and the only thing that matters is that all 148 SMs stream the same number of bytes and that the
+// pure HBM stream and the only thing that matters is that all SMs stream the same number of bytes and that the
 // fixed cost per launch (pipeline fill, epilogue, instruction fetch) is small.  Hence:
-//   * "swap AB": the weights sit on the UMMA M side (128 TMEM lanes = 128 output channels), the activations on the N
-//     side (BN = 16/32/64 columns), so a tiny m does not waste the 128-row MMA.
+//   * "swap AB": the weights sit on the wgmma M side (two m64 instructions = 128 output channels), the activations on the
+//     N side (BN = 16/32/64 columns), so a tiny m does not waste the 64-row MMA.
 //   * the tile height (weight rows per CTA, a multiple of 8 <= 128) and the split of K over a thread-block cluster of
 //     CS CTAs are chosen per shape so that tiles * CS ~ number of SMs, ONE tile per CTA, one wave (plan_decode).
 //   * K split inside the cluster is reduced through distributed shared memory: rank r owns the output columns
 //     j % CS == r, partial accumulators go to the owner with st.shared::cluster, one cluster barrier, no global traffic.
 //   * the weights never depend on the previous kernel: the TMA producer fills the whole ring BEFORE
 //     griddepcontrol.wait (programmatic dependent launch), so the stream overlaps the predecessor's tail.
-//   * the code is kept small on purpose (one tile, compile-time CS, rolled 16-column chunks): the general kernel of
-//     gemm_tc.cu measured ~12 k SASS instructions and was instruction-fetch bound in its epilogue (ncu: stall_no_inst).
+//   * the code is kept small on purpose (one tile, compile-time CS, rolled 16-column chunks), so that the epilogue is not
+//     bound by instruction fetch.
 //
 // Rounding points of the fused epilogue: DenseEpilogue / GluEpilogue / FloatEpilogue (common.cuh, gemm_common.cuh).
 #include <algorithm>
@@ -42,13 +42,14 @@ struct DecSmem {
   static constexpr int kA = NB * kTileM * kSwizzleBytes;       // weight bytes per stage (always 128-row slots)
   static constexpr int kB = BN * kSwizzleBytes;                // activation bytes per stage
   static constexpr int kStage = kA + kB;
-  static constexpr int kCtrl = 512;                            // barriers + TMEM slot
+  static constexpr int kCtrl = 512;                            // barriers
+  static constexpr int kAcc = acc_bytes(NB * BN);              // accumulators parked for the row-per-thread epilogue
   // per source rank and weight: (BN / 16) chunks x ceil(16 / cs) owned columns x 128 channels of 32-bit partials
   static size_t red_bytes(int cs) { return cs > 1 ? static_cast<size_t>(cs) * NB * (BN / 16) * ((16 + cs - 1) / cs) * kTileM * 4 : 0; }
-  static size_t bytes(int stages, int cs) { return static_cast<size_t>(stages) * kStage + kCtrl + red_bytes(cs) + 1024; }
+  static size_t bytes(int stages, int cs) { return kAcc + static_cast<size_t>(stages) * kStage + kCtrl + red_bytes(cs) + 1024; }
 };
 
-// T = output dtype, KIND = 0 s8 / 1 f16 / 2 bf16, BN = UMMA N (activation rows, zero padded), NB = 2 for gate+up,
+// T = output dtype, KIND = 0 s8 / 1 f16 / 2 bf16, BN = wgmma N (activation rows, zero padded), NB = 2 for gate+up,
 // CS = CTAs per tile (cluster size; K is split CS ways)
 template <typename T, int KIND, int BN, int NB, int CS>
 __global__ void __launch_bounds__(kTcThreads, 2)
@@ -57,8 +58,6 @@ __global__ void __launch_bounds__(kTcThreads, 2)
   using S = DecSmem<BN, NB>;
   constexpr int kElem = Elem<KIND>::bytes;
   constexpr int BK = kSwizzleBytes / kElem;
-  constexpr int kAccCols = BN * NB;
-  constexpr uint32_t kTmemCols = kAccCols <= 32 ? 32 : kAccCols <= 64 ? 64 : kAccCols <= 128 ? 128 : kAccCols <= 256 ? 256 : 512;
   // split-K ownership: inside every 16-column chunk, column j belongs to rank j % CS (slot j / CS of that chunk)
   constexpr int cp16 = (16 + CS - 1) / CS;             // owned columns per chunk
   constexpr int cpr = (BN / 16) * cp16;                // owned column slots per rank
@@ -66,11 +65,11 @@ __global__ void __launch_bounds__(kTcThreads, 2)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int nstages = p.stages;
-  uint8_t* ctrl = smem + nstages * S::kStage;
+  uint32_t* accs = reinterpret_cast<uint32_t*>(smem);                    // [NB * BN columns][kAccPitch]
+  uint8_t* ring = smem + S::kAcc;
+  uint8_t* ctrl = ring + nstages * S::kStage;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(ctrl);               // [kMaxStages]
   uint64_t* empty_bar = full_bar + kMaxStages;                           // [kMaxStages]
-  uint64_t* acc_bar = empty_bar + kMaxStages;                            // accumulators complete
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_bar + 1);
   uint32_t* red = reinterpret_cast<uint32_t*>(ctrl + S::kCtrl);          // [CS src][NB][cpr][128] (CS > 1)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -83,31 +82,26 @@ __global__ void __launch_bounds__(kTcThreads, 2)
   if (threadIdx.x == 0) {
     for (int s = 0; s < nstages; ++s) {
       mbar_init(full_bar + s, 1);
-      mbar_init(empty_bar + s, 1);
+      mbar_init(empty_bar + s, 4);                   // one arrive per consumer warp
     }
-    mbar_init(acc_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_slot, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   griddep_launch();
   if (CS > 1) cluster_arrive();                        // phase 1: every CTA of the cluster is alive
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ===== TMA producer =====
     if (elect_one()) {
       const uint32_t stage_tx = static_cast<uint32_t>(NB * p.tile_rows * kSwizzleBytes + S::kB);
       auto weights = [&](int s, int kb) {
-        uint8_t* sa = smem + s * S::kStage;
+        uint8_t* sa = ring + s * S::kStage;
         tma_load_2d(sa, &tm_w, full_bar + s, kb * BK, a0, kEvictFirst);
         if (NB == 2) tma_load_2d(sa + kTileM * kSwizzleBytes, &tm_w2, full_bar + s, kb * BK, a0, kEvictFirst);
       };
       auto acts = [&](int s, int kb) {
-        tma_load_2d(smem + s * S::kStage + S::kA, &tm_x, full_bar + s, kb * BK, 0, kEvictLast);
+        tma_load_2d(ring + s * S::kStage + S::kA, &tm_x, full_bar + s, kb * BK, 0, kEvictLast);
       };
       const int pre = min(nstages, nkb);
 #pragma unroll 1
@@ -127,35 +121,28 @@ __global__ void __launch_bounds__(kTcThreads, 2)
         acts(s, kb_lo + it);
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (elect_one()) {
-      constexpr uint32_t idesc = make_idesc<KIND>(BN);
-#pragma unroll 1
-      for (int it = 0; it < nkb; ++it) {
-        const int s = it % nstages;
-        mbar_wait(full_bar + s, (it / nstages) & 1);
-        tc_fence_after();
-        const uint32_t sa = smem_u32(smem + s * S::kStage);
-        const uint64_t db = make_smem_desc(sa + S::kA);
-#pragma unroll
-        for (int w = 0; w < NB; ++w) {
-          const uint64_t da = make_smem_desc(sa + w * kTileM * kSwizzleBytes);
-#pragma unroll
-          for (int k = 0; k < kSwizzleBytes / 32; ++k)      // +32 bytes of K inside the swizzle atom = +2 on the address field
-            umma<KIND>(tmem_base + w * BN, da + 2 * k, db + 2 * k, idesc, (it > 0 || k > 0) ? 1u : 0u);
-        }
-        umma_commit(empty_bar + s);
-      }
-      umma_commit(acc_bar);
-    }
   } else {
-    // ===== epilogue: thread = output channel (TMEM lane) =====
+    // ===== consumer warpgroup: wgmma over this CTA's K blocks, then the epilogue with thread = output channel =====
+    Acc<BN> acc[NB];
+#pragma unroll 1
+    for (int it = 0; it < nkb; ++it) {
+      const int s = it % nstages;
+      mbar_wait(full_bar + s, (it / nstages) & 1);
+      const uint32_t sa = smem_u32(ring + s * S::kStage);
+      wgmma_fence();
+#pragma unroll
+      for (int w = 0; w < NB; ++w) mma_block<KIND, BN>(acc[w], sa + w * kTileM * kSwizzleBytes, sa + S::kA, it == 0);
+      wgmma_commit();
+      wgmma_wait();
+      if (lane == 0) mbar_arrive(empty_bar + s);       // this warp's share of the stage has been read
+    }
+#pragma unroll
+    for (int w = 0; w < NB; ++w) acc_store<BN>(acc[w], accs + w * BN * kAccPitch);
+    epi_bar_sync();
     const int q = warp & 3;
     const int rloc = q * 32 + lane;
     const int64_t arow = static_cast<int64_t>(a0) + rloc;
     const bool row_ok = rloc < p.tile_rows && arow < p.n;
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
     griddep_wait();                                    // a_scale / residual come from the previous kernels
     float sw0 = 1.f, sw1 = 1.f, bias_t = 0.f;
     if (row_ok) {
@@ -165,14 +152,12 @@ __global__ void __launch_bounds__(kTcThreads, 2)
       }
       if (p.bias) bias_t = to_f32(static_cast<const T*>(p.bias)[arow]);
     }
-    mbar_wait(acc_bar, 0);
-    tc_fence_after();
     if constexpr (CS == 1) {
 #pragma unroll 1
       for (int c0 = 0; c0 < BN; c0 += 16) {
         uint32_t r[NB][16];
 #pragma unroll
-        for (int w = 0; w < NB; ++w) tmem_ld16x16(taddr + w * BN + c0, r[w]);
+        for (int w = 0; w < NB; ++w) acc_load<16>(accs + (w * BN + c0) * kAccPitch, rloc, r[w]);
         if (row_ok && c0 < p.m) dec_finish<T, KIND, NB, 16>(p, r, arow, c0, 1, 16, sw0, sw1, bias_t);
       }
     } else {
@@ -188,7 +173,7 @@ __global__ void __launch_bounds__(kTcThreads, 2)
       for (int c0 = 0; c0 < BN; c0 += 16) {
         uint32_t r[NB][16];
 #pragma unroll
-        for (int w = 0; w < NB; ++w) tmem_ld16x16(taddr + w * BN + c0, r[w]);
+        for (int w = 0; w < NB; ++w) acc_load<16>(accs + (w * BN + c0) * kAccPitch, rloc, r[w]);
         const uint32_t chunk_off = static_cast<uint32_t>((c0 / 16) * cp16 * kTileM * 4);
 #pragma unroll
         for (int j = 0; j < 16; ++j)
@@ -203,10 +188,10 @@ __global__ void __launch_bounds__(kTcThreads, 2)
 
   if constexpr (CS > 1) {
     __syncwarp();
-    if (warp < 2) cluster_wait();                      // phase 1 (the epilogue warps consumed it above)
+    if (warp == kProducerWarp) cluster_wait();         // phase 1 (the consumer warps consumed it above)
     cluster_arrive();                                  // phase 2: all partials have landed in their owners
     cluster_wait();
-    if (warp >= 2) {
+    if (warp < kProducerWarp) {
       const int q = warp & 3;
       const int rloc = q * 32 + lane;
       const int64_t arow = static_cast<int64_t>(a0) + rloc;
@@ -242,12 +227,6 @@ __global__ void __launch_bounds__(kTcThreads, 2)
     }
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
 }
 
 // ---- host side ----
@@ -282,7 +261,7 @@ template <int BN, int NB>
 int stages_for(int cs, int nkb) {
   using S = DecSmem<BN, NB>;
   const size_t cap = static_cast<size_t>(std::max(48, std::min(200, env_int("CT2B200_GEMM_SMEM_KB", 200)))) * 1024;
-  int st = static_cast<int>((cap - S::kCtrl - S::red_bytes(cs) - 1024) / S::kStage);
+  int st = static_cast<int>((cap - S::kAcc - S::kCtrl - S::red_bytes(cs) - 1024) / S::kStage);
   st = std::max(2, std::min(st, kMaxStages));
   return std::max(2, std::min(st, std::max(nkb, 2)));
 }
@@ -376,7 +355,7 @@ template <typename T, int KIND, int BN, int NB>
 bool run_decode(const void* x, const void* w, const void* w2, int64_t m, int64_t n, int64_t k, DecParams p,
                 cudaStream_t st, const NextWeights* next = nullptr) {
   constexpr int elem = Elem<KIND>::bytes;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   {
     static std::mutex mu;
@@ -417,18 +396,17 @@ bool run_decode_m(const void* x, const void* w, const void* w2, int64_t m, int64
   if (m <= 32) return run_decode<T, KIND, 32, NB>(x, w, w2, m, n, k, p, st, next);
   if (m <= 64) return run_decode<T, KIND, 64, NB>(x, w, w2, m, n, k, p, st, next);
   if constexpr (KIND == 0 && NB == 1) {
-    if (m <= 128) return run_decode<T, KIND, 128, NB>(x, w, w2, m, n, k, p, st, next);
-    if (m <= 256) return run_decode<T, KIND, 256, NB>(x, w, w2, m, n, k, p, st, next);
+    if (m <= 128) return run_decode<T, KIND, 128, NB>(x, w, w2, m, n, k, p, st, next);   // 128 accumulator registers per thread
   }
   return false;
 }
 
-// Rows this kernel takes.  Up to 64 it is the weight-streaming kernel of the decode step.  CT2B200_GEMM_DECODE_MAXM (up to 256)
-// also sends the small Dense layers of wide batches here (Transformer-base at batch x beam = 256: the whole weight matrix is a few
+// Rows this kernel takes.  Up to 64 it is the weight-streaming kernel of the decode step.  CT2B200_GEMM_DECODE_MAXM (up to 128: the accumulator registers of one warpgroup)
+// also sends the small Dense layers of wide batches here (Transformer-base at batch x beam = 128: the whole weight matrix is a few
 // hundred KB, the launch is latency-bound, and one lean tile per CTA on 8-32 SMs beats the persistent 128 x 256-tile kernel of
 // gemm_prefill.cu on 4-16); only matrices of at most 4 M weights, so that compute-bound prompt GEMMs never come here.
 int decode_max_m(int64_t n, int64_t k) {
-  static const int max_m = std::max(64, std::min(256, env_int("CT2B200_GEMM_DECODE_MAXM", CT2B200_DEFAULT_GEMM_DECODE_MAXM)));
+  static const int max_m = std::max(64, std::min(128, env_int("CT2B200_GEMM_DECODE_MAXM", CT2B200_DEFAULT_GEMM_DECODE_MAXM)));
   return n * k <= (4 << 20) ? max_m : 64;
 }
 
@@ -442,10 +420,7 @@ bool decode_kernel_enabled() {
 // The three entry points return false when the shape is not covered (m > 64, raw int32 output, more tiles than one
 // wave holds): the caller then uses the general persistent kernel of gemm_tc.cu.
 namespace {
-// The row pre-phase ([RMSNorm +] Quantize of the activations inside this kernel, behind a grid barrier) and the successor
-// prefetch into L2 were measured on the B200 (profiles/README.md, round 2): bit-identical, but SLOWER than the separate row
-// kernels under programmatic dependent launch (decode step 2.37 -> 2.63 ms at bsz 1, 3.22 -> 3.50 ms at bsz 32 — every CTA waits
-// at the barrier for the slowest row, and the extra code took the kernel from 70-86 to 168 registers).  They were removed;
+// The row pre-phase ([RMSNorm +] Quantize of the activations inside this kernel, behind a grid barrier) is not implemented:
 // callers that pass a RowPre get `false` and launch the row kernel themselves.
 bool set_row_pre(DecParams&, const RowPre* pre, const int8_t*, const float*, int64_t, int) { return !pre || pre->mode == 0; }
 }  // namespace

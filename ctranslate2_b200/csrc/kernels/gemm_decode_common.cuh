@@ -1,4 +1,4 @@
-// gemm_decode_common.cuh — pieces shared by the decode (weight-streaming) tcgen05 kernels: gemm_decode.cu (INT8 / f16
+// gemm_decode_common.cuh — pieces shared by the decode (weight-streaming) wgmma kernels: gemm_decode.cu (INT8 / f16
 // weights) and awq_decode.cu (AWQ-INT4 weights): fused epilogue of one output channel, cluster barriers, planner helpers.
 #pragma once
 
@@ -15,7 +15,7 @@ using namespace tc;
 
 constexpr int kMaxStages = 10;
 
-// defaults of the switchable kernels: 1 once a GPU session has validated them (profiles/README.md), 0 = opt-in until then
+// defaults of the switchable kernels (1 = on)
 #define CT2B200_DEFAULT_AWQ_DECODE 1
 #define CT2B200_DEFAULT_AWQ_GEMV 1
 #define CT2B200_DEFAULT_GEMM_DECODE_MAXM 64
@@ -43,17 +43,6 @@ template <int KIND> struct Elem { static constexpr int bytes = KIND == 0 ? 1 : 2
 static __device__ __noinline__ float dec_act(float x, int act) {
   if (act == CT2B200_ACT_SWISH) return __fdividef(x, 1.f + __expf(-x));
   return apply_act(x, act);
-}
-
-// 32 lanes x 16 columns of 32-bit accumulators -> 16 registers per thread
-__device__ __forceinline__ void tmem_ld16x16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 
 __device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
@@ -135,7 +124,7 @@ int max_clusters(K kernel, int cs, int threads, size_t smem, int sm_count) {
 inline int sm_count_of_current_device() {
   int dev = 0;
   cudaGetDevice(&dev);
-  static int cached_dev = -1, cached = 148;
+  static int cached_dev = -1, cached = 132;
   if (cached_dev != dev) {
     cudaDeviceGetAttribute(&cached, cudaDevAttrMultiProcessorCount, dev);
     cached_dev = dev;

@@ -1,4 +1,4 @@
-// gemm_prefill.cu — compute-bound GEMM of the prompt pass (many activation rows) on tcgen05, with the whole
+// gemm_prefill.cu — compute-bound GEMM of the prompt pass (many activation rows) on wgmma, with the whole
 // Dense epilogue fused: y[m, n] = epilogue(x[m, k] * W[n, k]^T).
 //
 // Replaces ops::Gemm (cuBLAS) + ops::Dequantize::dequantize_gemm_output + bias/activation + ops::Add / ops::Mul
@@ -7,13 +7,13 @@
 //
 // Shape of the problem: tensor-core bound.  One persistent CTA per SM walks 128 x 256 output tiles (GLU: 128 rows x
 // 128 gate + 128 up columns), M fastest so that the CTAs running at the same time share one weight tile in L2.
-//   warp 0      TMA producer: 4-stage ring of (A 128 x 128 B, B 256 x 128 B) operand slabs, SWIZZLE_128B
-//   warp 1      MMA issuer: tcgen05.mma kind::i8 / kind::f16, M = 128, N = 256, accumulators in TMEM
-//   warps 2-9   epilogue: TMEM is double buffered (2 x 256 columns), so the epilogue of tile i runs under the MMAs
-//               of tile i + 1.  Warp w reads TMEM lane quarter w % 4 and one half of the tile's columns; thread =
-//               output row, 32 columns per tcgen05.ld, 16-byte loads / stores of the residual and the result.
-// The general persistent kernel of gemm_tc.cu spent ~100 instructions per output element in a 4-warp epilogue and
-// was epilogue-bound for K = 4096 (ncu: stall_no_inst, 12 k SASS); this one needs ~6.
+//   warp 8      TMA producer: 3-stage ring of (A 128 x 128 B, B 256 x 128 B) operand slabs, SWIZZLE_128B; it runs ahead
+//               into the next tile while the consumers finish the current one
+//   warps 0-7   two consumer warpgroups; warpgroup h owns one half of the tile's output columns: per 32 bytes of K two m64
+//               wgmma row halves x its 64-column pieces (128 accumulator registers per thread), each K block waited for
+//               before the stage is handed back.  Then its epilogue: 32 accumulator columns at a time go through a
+//               [column][row] shared-memory buffer of the warpgroup to one output row per thread, 16-byte loads / stores
+//               of the residual and the result.  The epilogue of a tile does not overlap the MMAs of the next.
 // Rounding points: DenseEpilogue / GluEpilogue / FloatEpilogue (common.cuh, gemm_common.cuh).
 #include <algorithm>
 #include <cstdlib>
@@ -27,15 +27,35 @@ namespace {
 
 using namespace tc;
 
-constexpr int kThreads = 320;          // TMA warp, MMA warp, 8 epilogue warps
+constexpr int kThreads = 288;          // two consumer warpgroups (wgmma + epilogue of one half of the columns each), TMA warp
+constexpr int kTmaWarp = 8;
 constexpr int kBN = 256;               // accumulator columns per tile (NB = 2: 128 gate + 128 up)
-constexpr int kStages = 4;
+constexpr int kStages = 3;
 constexpr int kStageA = kTileM * kSwizzleBytes;      // 16 KB
 constexpr int kStageB = kBN * kSwizzleBytes;         // 32 KB
 constexpr int kStage = kStageA + kStageB;
-constexpr int kCtrl = 256;                           // barriers + TMEM slot
+constexpr int kCtrl = 256;                           // barriers
 constexpr int kScaleBytes = 2 * kBN * 4 * 2;         // [buf][256] weight scales + [buf][256] bias (fp32)
-constexpr size_t kSmemBytes = static_cast<size_t>(kStages) * kStage + kCtrl + kScaleBytes + 1024;
+constexpr int kChunk = 32;                           // accumulator columns handed to the row-per-thread epilogue at a time
+constexpr int kAccWg = acc_bytes(2 * kChunk);        // per warpgroup: one chunk of each of up to two weights
+constexpr size_t kSmemBytes = static_cast<size_t>(kStages) * kStage + 2 * kAccWg + kCtrl + kScaleBytes + 1024;
+
+// columns [C0, C0 + kChunk) of a warpgroup's accumulators -> dst[column][kAccPitch] (see acc_store)
+template <int C0, int BNH>
+__device__ __forceinline__ void store_chunk(const Acc<BNH>& c, uint32_t* dst) {
+  const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int j = 0; j < kChunk / 8; ++j) {
+      uint32_t* q = dst + (j * 8 + (l & 3) * 2) * kAccPitch + h * 64 + w * 16 + (l >> 2);
+      const uint32_t* d = c.d[h][C0 / 64] + 4 * ((C0 % 64) / 8 + j);
+      q[0] = d[0];
+      q[kAccPitch] = d[1];
+      q[8] = d[2];
+      q[kAccPitch + 8] = d[3];
+    }
+}
 
 struct PreParams {
   int64_t m, n;          // output rows / channels (NB = 2: n = channels of ONE of the two weights)
@@ -59,6 +79,7 @@ __device__ __noinline__ float pre_act(float x, int act) {
 }
 
 __device__ __forceinline__ void epi_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+__device__ __forceinline__ void wg_sync(int half) { asm volatile("bar.sync %0, 128;" ::"r"(2 + half) : "memory"); }
 
 // T = output dtype (2 or 4 bytes), KIND = 0 s8 / 1 f16 / 2 bf16, NB = 2: gate/up fusion, BN = accumulator columns per tile:
 // 256, or 64 for Dense layers whose 128 x 256 tiles would occupy a handful of SMs (Transformer-base at 256 rows: 4 tiles; the
@@ -75,12 +96,10 @@ __global__ void __launch_bounds__(kThreads, 1)
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* ctrl = smem + kStages * kStage;
+  uint8_t* accs = smem + kStages * kStage;                     // [warpgroup][2 * kChunk columns][kAccPitch]
+  uint8_t* ctrl = accs + 2 * kAccWg;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(ctrl);     // [kStages]
   uint64_t* empty_bar = full_bar + kStages;                    // [kStages]
-  uint64_t* acc_full = empty_bar + kStages;                    // [2]
-  uint64_t* acc_empty = acc_full + 2;                          // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(acc_empty + 2);
   float* s_scale = reinterpret_cast<float*>(ctrl + kCtrl);     // [2][256]
   float* s_bias = s_scale + 2 * kBN;                           // [2][256]
 
@@ -91,23 +110,15 @@ __global__ void __launch_bounds__(kThreads, 1)
   if (threadIdx.x == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(full_bar + s, 1);
-      mbar_init(empty_bar + s, 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(acc_full + b, 1);
-      mbar_init(acc_empty + b, 8);                 // one arrive per epilogue warp
+      mbar_init(empty_bar + s, 8);                 // one arrive per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_slot, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   griddep_launch();
 
-  if (warp == 0) {
+  if (warp == kTmaWarp) {
     // ===== TMA producer =====
     if (elect_one()) {
       griddep_wait();                              // the activations come from the previous kernel
@@ -129,40 +140,15 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (elect_one()) {
-      constexpr uint32_t idesc = make_idesc<KIND>(BN);
-      int it = 0, seq = 0;
-#pragma unroll 1
-      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++seq) {
-        const int buf = seq & 1;
-        if (seq >= 2) mbar_wait(acc_empty + buf, ((seq >> 1) & 1) ^ 1);   // the epilogue drained this buffer
-        tc_fence_after();
-        const uint32_t acc = tmem_base + buf * BN;
-#pragma unroll 1
-        for (int kb = 0; kb < KB; ++kb, ++it) {
-          const int s = it % kStages;
-          mbar_wait(full_bar + s, (it / kStages) & 1);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + s * kStage);
-          const uint64_t da = make_smem_desc(sa);
-          const uint64_t db = make_smem_desc(sa + kStageA);
-#pragma unroll
-          for (int k = 0; k < kSwizzleBytes / 32; ++k)
-            umma<KIND>(acc, da + 2 * k, db + 2 * k, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          umma_commit(empty_bar + s);
-        }
-        umma_commit(acc_full + buf);
-      }
-    }
   } else {
-    // ===== epilogue =====
+    // ===== consumer warpgroups: wgmma over the K blocks of a tile, then its epilogue =====
     griddep_wait();
-    const int ew = warp - 2;                       // 0..7
-    const int q = warp & 3;                        // TMEM lane quarter
-    const int half = ew >> 2;                      // which half of the output columns
-    const int et = threadIdx.x - 64;               // 0..255
+    const int q = warp & 3;
+    const int half = warp >> 2;                    // which half of the output columns this warpgroup computes
+    const int et = threadIdx.x;                    // 0..255
+    uint32_t* my_acc = reinterpret_cast<uint32_t*>(accs + half * kAccWg);
+    constexpr int kAccN = NB == 2 ? kOutCols / 2 : BN / 2;     // accumulator columns per weight and warpgroup
+    int it = 0;
     const int rloc = q * 32 + lane;
     constexpr int kColsPerWarp = kOutCols / 2;     // 128 (NB = 1) or 64 (NB = 2)
     constexpr int kVec = 16 / sizeof(T);           // elements per 16-byte access
@@ -195,17 +181,39 @@ __global__ void __launch_bounds__(kThreads, 1)
       }
       float sa = 1.f;
       if constexpr (KIND == 0) sa = row_ok ? p.a_scale[row] : 1.f;      // written by the previous kernel: not through the read-only path (build.py)
+      Acc<kAccN> acc[NB];
+#pragma unroll 1
+      for (int kb = 0; kb < KB; ++kb, ++it) {
+        const int s = it % kStages;
+        mbar_wait(full_bar + s, (it / kStages) & 1);
+        const uint32_t sa = smem_u32(smem + s * kStage);
+        const uint32_t sb = sa + kStageA + half * kAccN * kSwizzleBytes;
+        wgmma_fence();
+#pragma unroll
+        for (int w = 0; w < NB; ++w) mma_block<KIND, kAccN>(acc[w], sa, sb + w * kWRows * kSwizzleBytes, kb == 0);
+        wgmma_commit();
+        wgmma_wait();
+        if (lane == 0) mbar_arrive(empty_bar + s);  // this warp's share of the stage has been read
+      }
       epi_sync();                                  // column constants of this tile are in place
-      mbar_wait(acc_full + buf, (seq >> 1) & 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + buf * BN + (static_cast<uint32_t>(q * 32) << 16);
       T* yrow = static_cast<T*>(p.y) + row * p.ldy + n0;
       const T* rrow = p.residual ? static_cast<const T*>(p.residual) + row * p.ldy + n0 : nullptr;
-#pragma unroll 1
-      for (int c0 = half * kColsPerWarp; c0 < (half + 1) * kColsPerWarp; c0 += 32) {
+#pragma unroll
+      for (int cc = 0; cc < kColsPerWarp; cc += kChunk) {
+        const int c0 = half * kColsPerWarp + cc;
+        // this chunk of the fragments -> shared memory -> one row per thread
+        wg_sync(half);
+#pragma unroll
+        for (int w = 0; w < NB; ++w) {
+          if (cc == 0) store_chunk<0>(acc[w], my_acc + w * kChunk * kAccPitch);
+          if (cc == 32) store_chunk<32 % kAccN>(acc[w], my_acc + w * kChunk * kAccPitch);
+          if (cc == 64) store_chunk<64 % kAccN>(acc[w], my_acc + w * kChunk * kAccPitch);
+          if (cc == 96) store_chunk<96 % kAccN>(acc[w], my_acc + w * kChunk * kAccPitch);
+        }
+        wg_sync(half);
         // The residual of the whole 32-column chunk is requested before the accumulators are read.  y may alias the residual
         // (in-place x += Dense(...)), so loads left between the stores below stay in program order: one L2 round trip per
-        // 16-byte vector, 16 per thread and tile (the 128 x 256 tile of a 512-wide Dense took 15.7 us, most of it this chain).
+        // 16-byte vector, 16 per thread and tile.
         Vec16<T> res[32 / kVec];
         if constexpr (NB == 1) {
           if (rrow && row_ok) {
@@ -215,10 +223,10 @@ __global__ void __launch_bounds__(kThreads, 1)
           }
         }
         uint32_t r0[32];
-        tmem_ld32(taddr + c0, r0);
+        acc_load<32>(my_acc, rloc, r0);
         if constexpr (NB == 2) {
           uint32_t r1[32];
-          tmem_ld32(taddr + kOutCols + c0, r1);
+          acc_load<32>(my_acc + kChunk * kAccPitch, rloc, r1);
           if (row_ok) {
 #pragma unroll
             for (int v0 = 0; v0 < 32; v0 += kVec) {
@@ -263,18 +271,7 @@ __global__ void __launch_bounds__(kThreads, 1)
           }
         }
       }
-      // all TMEM reads of this buffer are complete (tcgen05.wait::ld inside tmem_ld32): hand it back
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc_empty + buf);
     }
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -304,7 +301,7 @@ void launch_prefill(const void* x, const void* w, const void* w2, int64_t m, int
                     cudaStream_t st) {
   int dev = 0;
   cudaGetDevice(&dev);
-  static int cached_dev = -1, cached_sms = 148;
+  static int cached_dev = -1, cached_sms = 132;
   if (cached_dev != dev) {
     cudaDeviceGetAttribute(&cached_sms, cudaDevAttrMultiProcessorCount, dev);
     cached_dev = dev;

@@ -1,7 +1,7 @@
 // gemm_s8_mma.cu — INT8 GEMM C[m,n] = A[m,k] · B[n,k]^T (int32 accumulate) with the fused Dense
 // epilogue, on legacy warp-level tensor-core instructions (mma.sync.m16n8k32.s8) with a cp.async
-// multi-stage pipeline.  This is the portable fallback / cross-check of the tcgen05 kernel in
-// gemm_tc.cu (SURVEY §0 fact 10 asks for one); the engine prefers tcgen05.
+// multi-stage pipeline.  This is the portable fallback / cross-check of the wgmma kernel in
+// gemm_tc.cu (SURVEY §0 fact 10 asks for one); the engine prefers wgmma.
 //
 // Replaces: cublasGemmEx(CUDA_R_8I) src/cuda/primitives.cu:571-597 + dequantize_gemm_output_kernel
 // src/ops/dequantize_gpu.cu:30-121 + ops::Add / ops::Mul (src/layers/common.cc:392-401, transformer.cc:31-37).

@@ -1,8 +1,8 @@
-// gemm_tc.cu — the GENERAL tcgen05 GEMM (first tensor-core kernel of this repo, now the fallback of the two
-// specialised ones): tcgen05.mma (kind::i8 / kind::f16) with TMA-staged, 128B-swizzled operand tiles in shared
-// memory, accumulators in TMEM, fused Dense epilogue read back with tcgen05.ld.
+// gemm_tc.cu — the GENERAL wgmma GEMM (the fallback of the two specialised ones): wgmma (s8 / f16 / bf16) with
+// TMA-staged, 128B-swizzled operand tiles in shared memory, accumulators in the registers of one warpgroup, fused
+// Dense epilogue (one output row per thread, fed through a shared-memory transpose of the fragments).
 //   * gemm_s8_tc / gemm_s8_glu_tc / gemm_f16_tc first try gemm_decode.cu (m <= 64, one tile per CTA, cluster/DSMEM
-//     split-K) and gemm_prefill.cu (m > 64, double-buffered TMEM, 8 epilogue warps) and only land here for what those
+//     split-K) and gemm_prefill.cu (m > 64, two consumer warpgroups) and only land here for what those
 //     do not cover: raw int32 output (ops::Gemm), N tiles beyond one wave at m <= 64 (the 128256-row lm_head),
 //     unaligned rows.
 //   * persistent stream-K over (tile, K block) units, "swap-AB" for m <= 64, cluster / partition / whole-tile modes,
@@ -10,8 +10,8 @@
 // Replaces cublasGemmEx s8/f16/bf16 (reference src/cuda/primitives.cu:485-597) + Dequantize epilogue
 // (src/ops/dequantize_gpu.cu:30-121) + ops::Add/ops::Mul (src/layers/common.cc:392-401, transformer.cc:31-37).
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM owner + MMA issuer (one elected lane),
-// warps 2..5 = epilogue (warp w reads TMEM lanes 32*(w%4) ..+31).
+// Warp roles (160 threads): warps 0..3 = consumer warpgroup (wgmma, then the epilogue: thread t owns tile row t),
+// warp 4 = TMA producer (one elected lane).
 #include <cuda.h>
 #include <cudaTypedefs.h>
 
@@ -59,8 +59,9 @@ struct TcSmem {
   static constexpr int kA = kTileM * kSwizzleBytes * (kSwap ? NB : 1);     // M-side bytes per stage
   static constexpr int kB = BN * kSwizzleBytes * (kSwap ? 1 : NB);         // N-side bytes per stage
   static constexpr int kStage = kA + kB;
-  static constexpr int kStages = (200 * 1024 / kStage) > 8 ? 8 : (200 * 1024 / kStage);
-  static constexpr size_t kBytes = static_cast<size_t>(kStages) * kStage + 1024 /*align*/ + 256 /*barriers*/;
+  static constexpr int kAcc = acc_bytes(NB * BN);                          // accumulators parked for the epilogue
+  static constexpr int kStages = ((200 * 1024 - kAcc) / kStage) > 8 ? 8 : ((200 * 1024 - kAcc) / kStage);
+  static constexpr size_t kBytes = kAcc + static_cast<size_t>(kStages) * kStage + 1024 /*align*/ + 256 /*barriers*/;
 };
 
 // Activation out of line: the epilogue is unrolled over the columns of a chunk, and inlining erff/tanhf/expf
@@ -169,25 +170,14 @@ __device__ __forceinline__ void epi_finish(const TcParams& p, const uint32_t (&r
   }
 }
 
-// 32 lanes x 16 columns of 32-bit accumulators -> 16 registers per thread
-__device__ __forceinline__ void tmem_ld16x(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-
 // Persistent "stream-K" GEMM: the work is the list of (output tile, K block) units, tile-major; CTA c of P
 // owns the contiguous unit range [c*U/P, (c+1)*U/P), so every SM streams the same number of bytes and the TMA
 // ring never drains between tiles.  A tile whose K range is covered by one CTA is finished by that CTA
-// straight from TMEM; a tile shared by several CTAs is reduced through the zeroed scratch (integer
+// straight from its accumulators; a tile shared by several CTAs is reduced through the zeroed scratch (integer
 // red.global.add => bit-exact, order independent) and finished by the last arriver (ticket).
-// Accumulators are double-buffered in TMEM so the epilogue of one segment overlaps the MMAs of the next.
+// The TMA producer runs ahead into the next segment while the warpgroup finishes the current one.
 //
-// T = output dtype, KIND = 0 s8 / 1 f16 / 2 bf16, BN = UMMA N, NB = weight matrices (2 = GLU),
+// T = output dtype, KIND = 0 s8 / 1 f16 / 2 bf16, BN = wgmma N (BN * NB <= 128 accumulator registers), NB = weight matrices (2 = GLU),
 // kSwap = weights on the M side (decode).
 template <typename T, int KIND, int BN, int NB, bool kSwap>
 __global__ void __launch_bounds__(kTcThreads, 1)
@@ -196,20 +186,15 @@ __global__ void __launch_bounds__(kTcThreads, 1)
   using S = TcSmem<BN, NB, kSwap>;
   constexpr int kElem = KindTraits<KIND>::kElem;
   constexpr int BK = kSwizzleBytes / kElem;            // elements of K per stage
-  constexpr int kUmmaK = 32 / kElem;                   // elements of K per MMA
   constexpr int kStages = S::kStages;
-  constexpr int kAccCols = BN * NB;                    // TMEM columns per accumulator buffer
-  constexpr uint32_t kTmemCols = (2 * kAccCols) <= 32 ? 32 : (2 * kAccCols) <= 64 ? 64 : (2 * kAccCols) <= 128 ? 128
-                               : (2 * kAccCols) <= 256 ? 256 : 512;
-  static_assert(BN % 16 == 0 && BN >= 16 && BN <= 256 && 2 * kAccCols <= 512, "invalid UMMA N");
+  static_assert(BN * NB <= 128 && kStages >= 2, "the accumulators of a tile live in the registers of one warpgroup");
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + p.stages * S::kStage);      // [kStages] (p.stages used)
+  uint32_t* accs = reinterpret_cast<uint32_t*>(smem);                                 // [NB * BN columns][kAccPitch]
+  uint8_t* ring = smem + S::kAcc;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(ring + p.stages * S::kStage);      // [kStages] (p.stages used)
   uint64_t* empty_bar = full_bar + kStages;
-  uint64_t* tmem_full_bar = empty_bar + kStages;       // [2]
-  uint64_t* tmem_empty_bar = tmem_full_bar + 2;        // [2]
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(tmem_empty_bar + 2);
   __shared__ int s_last;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -254,23 +239,15 @@ __global__ void __launch_bounds__(kTcThreads, 1)
   if (threadIdx.x == 0) {
     for (int s = 0; s < p.stages; ++s) {
       mbar_init(full_bar + s, 1);
-      mbar_init(empty_bar + s, 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(tmem_full_bar + b, 1);
-      mbar_init(tmem_empty_bar + b, 4);               // one arrive per epilogue warp
+      mbar_init(empty_bar + s, 4);                    // one arrive per consumer warp
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 1) tmem_alloc(tmem_slot, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
   griddep_launch();                                 // the next kernel may be scheduled; it waits on our completion
   // cluster mode: reduction buffer behind the barriers; [src rank][plane][owned column][128 rows] of 32-bit partials
-  uint32_t* red = reinterpret_cast<uint32_t*>(smem + nstages * S::kStage + 512);
+  uint32_t* red = reinterpret_cast<uint32_t*>(ring + nstages * S::kStage + 512);
   const int cpr = CS >= 2 ? (BN + CS - 1) / CS : 0;   // columns owned per rank (column j belongs to rank j % CS)
   if (CS >= 2) asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");   // peers are alive before DSMEM traffic
 
@@ -281,7 +258,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
   const uint64_t pol_a = kSwap ? kEvictFirst : kEvictLast;   // weights stream once; activations are reused
   const uint64_t pol_b = kSwap ? kEvictLast : kEvictFirst;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ===== TMA producer =====
     if (elect_one()) {
       int it = 0;
@@ -292,7 +269,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
       // griddepcontrol.wait (so the pipeline fills during the predecessor's tail); the activation tiles after it.
       const int64_t prefill = min(static_cast<int64_t>(nstages), u_end - u_begin);
       auto issue = [&](int s, int kc, bool weights, bool acts) {
-        uint8_t* sa = smem + s * S::kStage;
+        uint8_t* sa = ring + s * S::kStage;
         uint8_t* sb = sa + S::kA;
         if (kSwap) {
           if (weights) {
@@ -338,63 +315,25 @@ __global__ void __launch_bounds__(kTcThreads, 1)
         }
       }
     }
-  } else if (warp == 1) {
-    // ===== MMA issuer =====
-    if (elect_one()) {
-      constexpr uint32_t idesc = make_idesc<KIND>(BN);
-      int it = 0, seg = 0;
-      for (int64_t u = u_begin; u < u_end; ++seg) {
-        const int64_t tile = u / KB;
-        const int kb0 = static_cast<int>(u - tile * KB);
-        const int kb1 = static_cast<int>(min(KB, static_cast<int64_t>(kb0) + (u_end - u)));
-        const int buf = seg & 1;
-        mbar_wait(tmem_empty_bar + buf, ((seg >> 1) & 1) ^ 1);       // epilogue drained this buffer
-        tc_fence_after();
-        const uint32_t acc = tmem_base + buf * kAccCols;
-        for (int kb = kb0; kb < kb1; ++kb, ++it) {
-          const int s = it % nstages;
-          const uint32_t ph = (it / nstages) & 1;
-          mbar_wait(full_bar + s, ph);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + s * S::kStage);
-          const uint32_t sb = sa + S::kA;
-#pragma unroll
-          for (int w = 0; w < NB; ++w) {
-            const uint64_t da = make_smem_desc(sa + (kSwap ? w * kTileM * kSwizzleBytes : 0));
-            const uint64_t db = make_smem_desc(sb + (kSwap ? 0 : w * BN * kSwizzleBytes));
-#pragma unroll
-            for (int k = 0; k < BK / kUmmaK; ++k) {
-              // advancing K inside the 128B swizzle atom = +32 bytes on the start address (>>4 => +2)
-              umma<KIND>(acc + w * BN, da + 2 * k, db + 2 * k, idesc, (kb > kb0 || k > 0) ? 1u : 0u);
-            }
-          }
-          umma_commit(empty_bar + s);               // frees the smem stage when these MMAs retire
-        }
-        umma_commit(tmem_full_bar + buf);           // this segment's accumulators are complete
-        u += kb1 - kb0;
-      }
-    }
   } else {
-    // ===== epilogue warps =====
+    // ===== consumer warpgroup: wgmma over a segment's K blocks, then its epilogue =====
     griddep_wait();                                 // scales / residual come from the previous kernels
-    const int q = warp & 3;                         // TMEM lane quarter this warp may access
-    const int et = threadIdx.x - 64;                // 0..127 among the epilogue threads (== q * 32 + lane)
+    const int q = warp & 3;
+    const int et = threadIdx.x;                     // 0..127 among the consumer threads (== q * 32 + lane)
     const int64_t ldw = kSwap ? p.rows_a : p.rows_b;                 // row pitch of the [m, n] scratch plane
     const int64_t plane = p.rows_a * p.rows_b;
     constexpr int kC = 16;                          // columns per chunk (rolled loop over chunks keeps the code small)
-    int seg = 0;
-    for (int64_t u = u_begin; u < u_end; ++seg) {
+    int it = 0;
+    for (int64_t u = u_begin; u < u_end;) {
       const int64_t tile = u / KB;
       const int kb0 = static_cast<int>(u - tile * KB);
       const int kb1 = static_cast<int>(min(KB, static_cast<int64_t>(kb0) + (u_end - u)));
       u += kb1 - kb0;
       const int64_t a0 = (tile % p.tiles_a) * kTileM;
       const int64_t b0 = (tile / p.tiles_a) * BN;
-      const int buf = seg & 1;
       const bool direct = kb0 == 0 && kb1 == KB;
-      const int rloc = q * 32 + lane;               // tile row owned by this thread (= its TMEM lane)
+      const int rloc = q * 32 + lane;               // tile row owned by this thread
       const int64_t arow = a0 + rloc;
-      const uint32_t taddr = tmem_base + buf * kAccCols + (static_cast<uint32_t>(q * 32) << 16);
       // partial tiles are parked in per-CTA slots (plain coalesced stores: no atomics, nothing to re-zero, no
       // same-address contention) and summed by the last arriver in CTA order (deterministic for the float kinds)
       constexpr int64_t kSlot = static_cast<int64_t>(NB) * kTileM * BN;
@@ -403,9 +342,28 @@ __global__ void __launch_bounds__(kTcThreads, 1)
       int c_lo = 0, c_hi = 0;
       EpiInputs<NB, kC> ein;
       if (direct) epi_load<T, KIND, NB, kSwap, kC>(p, arow, b0, ein);   // issued while the MMAs of this segment run
-      mbar_wait(tmem_full_bar + buf, (seg >> 1) & 1);
-      tc_fence_after();
-      // pass 0: accumulators from TMEM -> epilogue (tile owned by this CTA alone) or -> scratch (shared tile);
+      {
+        Acc<BN> acc[NB];
+#pragma unroll 1
+        for (int kb = kb0; kb < kb1; ++kb, ++it) {
+          const int s = it % nstages;
+          mbar_wait(full_bar + s, (it / nstages) & 1);
+          const uint32_t sa = smem_u32(ring + s * S::kStage);
+          const uint32_t sb = sa + S::kA;
+          wgmma_fence();
+#pragma unroll
+          for (int w = 0; w < NB; ++w)
+            mma_block<KIND, BN>(acc[w], sa + (kSwap ? w * kTileM * kSwizzleBytes : 0), sb + (kSwap ? 0 : w * BN * kSwizzleBytes), kb == kb0);
+          wgmma_commit();
+          wgmma_wait();
+          if (lane == 0) mbar_arrive(empty_bar + s);  // this warp's share of the stage has been read
+        }
+        epi_bar_sync();                               // the previous segment's rows have been read out of accs
+#pragma unroll
+        for (int w = 0; w < NB; ++w) acc_store<BN>(acc[w], accs + w * BN * kAccPitch);
+        epi_bar_sync();
+      }
+      // pass 0: accumulators -> epilogue (tile owned by this CTA alone) or -> scratch (shared tile);
       // pass 1 (last arriver of a shared tile only): reduced accumulators from the scratch -> epilogue.
 #pragma unroll 1
       for (int pass = 0; pass < 2; ++pass) {
@@ -415,12 +373,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
           if (pass == 0) {
             if (direct && c0 > 0) epi_load<T, KIND, NB, kSwap, kC>(p, arow, b0 + c0, ein);
 #pragma unroll
-            for (int w = 0; w < NB; ++w) tmem_ld16x(taddr + w * BN + c0, r[w]);
-            if (c0 + kC >= BN) {                    // everything is in registers: hand the TMEM buffer back
-              tc_fence_before();
-              __syncwarp();
-              if (lane == 0) mbar_arrive(tmem_empty_bar + buf);
-            }
+            for (int w = 0; w < NB; ++w) acc_load<kC>(accs + (w * BN + c0) * kAccPitch, rloc, r[w]);
           } else {
             // the epilogue inputs and the reduced accumulators are requested together: one memory round trip
             epi_load<T, KIND, NB, kSwap, kC>(p, arow, b0 + c0, ein);
@@ -492,10 +445,10 @@ __global__ void __launch_bounds__(kTcThreads, 1)
   if (CS >= 2) {
     // every thread of the cluster meets here: all partials have landed in their owners' shared memory
     __syncwarp();
-    if (warp < 2) asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");     // pending start-up phase
+    if (warp == kProducerWarp || u_end <= u_begin) asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");     // pending start-up phase
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
     asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-    if (warp >= 2 && u_end > u_begin) {
+    if (warp < kProducerWarp && u_end > u_begin) {
       // each CTA finishes the columns it owns: sum the CS partials in rank order (deterministic), fused epilogue
       constexpr int kC2 = 16;
       const int q = warp & 3;
@@ -528,12 +481,6 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     }
   }
 
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
-  }
 }
 
 // ---- host side ----
@@ -571,7 +518,7 @@ void launch_tc(const void* x, const void* w, const void* w2, int64_t m, int64_t 
   int max_stages = S::kStages;
   if (kSwap && smem_cap_kb > 0) max_stages = std::max(2, std::min<int>(S::kStages, smem_cap_kb * 1024 / S::kStage));
   p.stages = max_stages;
-  size_t smem_bytes = static_cast<size_t>(max_stages) * S::kStage + 1024 + 256;
+  size_t smem_bytes = S::kAcc + static_cast<size_t>(max_stages) * S::kStage + 1024 + 256;
   static const int mode = [] { const char* e = std::getenv("CT2B200_GEMM_SPLIT"); return e ? std::atoi(e) : 0; }();   // 1 = stream-K, 2 = partition
   if (kSwap && !force_whole && mode == 0 && tiles < wsp.sm_count) {
     // Decode GEMMs (fewer tiles than SMs).  Split-K through global memory costs several dependent L2 round trips in
@@ -580,18 +527,18 @@ void launch_tc(const void* x, const void* w, const void* w2, int64_t m, int64_t 
     //    partial accumulators are exchanged through distributed shared memory (no global traffic, one cluster barrier);
     //  * otherwise whole tiles (no reduction at all) on as many SMs as there are tiles.
     int cs = static_cast<int>(wsp.sm_count / tiles);
-    if (cs > 4) cs = 4;                                      // clusters of 4 still fill 132 of 148 SMs
-    if (cs == 3 && tiles * 3 > 132) cs = 2;                  // keep every cluster co-resident
+    if (cs > 4) cs = 4;
+    if (cs == 3 && tiles * 3 > wsp.sm_count / 4 * 4) cs = 2; // odd clusters do not tile the GPCs: leave a cluster of 4 SMs spare so all are co-resident (not measured on H100)
     while (cs >= 2 && p.kb_total < 2 * cs) --cs;
     if (cs >= 2) {
       const size_t red_bytes = static_cast<size_t>(cs) * NB * ((BN + cs - 1) / cs) * kTileM * 4;
       int stages = max_stages;
-      while (stages > 2 && static_cast<size_t>(stages) * S::kStage + 1024 + 512 + red_bytes > 226 * 1024) --stages;
+      while (stages > 2 && S::kAcc + static_cast<size_t>(stages) * S::kStage + 1024 + 512 + red_bytes > 226 * 1024) --stages;
       p.cluster_s = cs;
       p.stages = stages;
       p.whole_tiles = 0;
       ctas = tiles * cs;
-      smem_bytes = static_cast<size_t>(stages) * S::kStage + 1024 + 512 + red_bytes;
+      smem_bytes = S::kAcc + static_cast<size_t>(stages) * S::kStage + 1024 + 512 + red_bytes;
     } else {
       p.whole_tiles = 1;
       ctas = tiles;
@@ -633,8 +580,8 @@ void launch_tc_shape(const void* x, const void* w, const void* w2, int64_t m, in
   if (m <= 16) launch_tc<T, KIND, 16, NB, true>(x, w, w2, m, n, k, p, st);
   else if (m <= 32) launch_tc<T, KIND, 32, NB, true>(x, w, w2, m, n, k, p, st);
   else if (m <= 64) launch_tc<T, KIND, 64, NB, true>(x, w, w2, m, n, k, p, st);
-  else if constexpr (NB == 2) launch_tc<T, KIND, 128, NB, false>(x, w, w2, m, n, k, p, st);
-  else launch_tc<T, KIND, 256, NB, false>(x, w, w2, m, n, k, p, st);
+  else if constexpr (NB == 2) launch_tc<T, KIND, 64, NB, false>(x, w, w2, m, n, k, p, st);
+  else launch_tc<T, KIND, 128, NB, false>(x, w, w2, m, n, k, p, st);
 }
 
 }  // namespace

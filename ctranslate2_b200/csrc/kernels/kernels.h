@@ -54,7 +54,7 @@ void launch_tp_reduce(const TpLink& tp, int buf, int sync_idx, void* x, int64_t 
 void launch_tp_quantize_rows(const TpLink& tp, int slot, int sync_idx, const void* x, int64_t rows, int64_t cols, int8_t* q,
                              float* scale, int dtype, cudaStream_t st);
 
-// gemm_tc.cu (tcgen05) — gemm_s8_mma.cu declarations live in gemm_common.cuh
+// gemm_tc.cu (wgmma) — gemm_s8_mma.cu declarations live in gemm_common.cuh
 void gemm_s8_tc(const int8_t* A, const int8_t* B, int64_t M, int64_t N, int64_t K, const DenseEpilogue& epi,
                 int dtype, cudaStream_t st);
 void gemm_s8_glu_tc(const int8_t* A, const int8_t* Bgate, const int8_t* Bup, int64_t M, int64_t N, int64_t K,
@@ -79,7 +79,7 @@ struct NextWeights {
   const void* w2 = nullptr;
   int64_t n = 0, k = 0;
 };
-// gemm_decode.cu (tcgen05, m <= 64): false = shape (or pre-phase) not covered, use the general kernel (+ separate row kernel)
+// gemm_decode.cu (wgmma, m <= 64): false = shape (or pre-phase) not covered, use the general kernel (+ separate row kernel)
 bool gemm_s8_decode(const int8_t* A, const int8_t* B, int64_t M, int64_t N, int64_t K, const DenseEpilogue& epi,
                     int dtype, cudaStream_t st, const RowPre* pre = nullptr, const NextWeights* next = nullptr);
 bool gemm_s8_glu_decode(const int8_t* A, const int8_t* Bgate, const int8_t* Bup, int64_t M, int64_t N, int64_t K,
@@ -88,7 +88,7 @@ bool gemm_s8_glu_decode(const int8_t* A, const int8_t* Bgate, const int8_t* Bup,
 bool gemm_f16_decode(const void* A, const void* B, const void* bias, const void* residual, int act, int64_t M,
                      int64_t N, int64_t K, void* C, int dtype, cudaStream_t st);
 
-// gemm_prefill.cu (tcgen05, m > 64, compute bound): false = shape not covered
+// gemm_prefill.cu (wgmma, m > 64, compute bound): false = shape not covered
 bool gemm_s8_prefill(const int8_t* A, const int8_t* B, int64_t M, int64_t N, int64_t K, const DenseEpilogue& epi,
                      int dtype, cudaStream_t st);
 bool gemm_s8_glu_prefill(const int8_t* A, const int8_t* Bgate, const int8_t* Bup, int64_t M, int64_t N, int64_t K,

@@ -1,6 +1,7 @@
-// tc_common.cuh — inline-PTX wrappers shared by the tcgen05 kernels (gemm_tc.cu, awq.cu): mbarrier, TMA
-// (cp.async.bulk.tensor), TMEM allocation / tcgen05.ld, tcgen05.mma + commit, UMMA descriptors.
-// Bit layouts follow cute::UMMA::SmemDescriptor / InstrDescriptor (CUTLASS, cute/arch/mma_sm100_desc.hpp).
+// tc_common.cuh — inline-PTX wrappers shared by the wgmma kernels (gemm_tc.cu, gemm_decode.cu, gemm_prefill.cu, awq.cu,
+// awq_decode.cu): mbarrier, TMA (cp.async.bulk.tensor), wgmma with its shared-memory descriptors, and the hand-over of
+// the register accumulators to the row-per-thread epilogues.
+// Bit layouts follow cute::GmmaDescriptor (CUTLASS, cute/arch/mma_sm90_desc.hpp).
 #pragma once
 
 #include <cuda.h>
@@ -13,8 +14,9 @@
 namespace ct2b200 {
 namespace tc {
 
-constexpr int kTcThreads = 192;
-constexpr int kTileM = 128;              // UMMA M
+constexpr int kTcThreads = 160;          // warps 0-3 = the consumer warpgroup (wgmma + epilogue), warp 4 = TMA producer
+constexpr int kProducerWarp = 4;
+constexpr int kTileM = 128;              // tile rows: two m64 wgmma instructions
 constexpr int kSwizzleBytes = 128;       // bytes of K per smem row (= one 128B swizzle atom)
 constexpr uint64_t kEvictFirst = 0x12F0000000000000ull;
 constexpr uint64_t kEvictLast = 0x14F0000000000000ull;
@@ -29,9 +31,8 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
 }
 // One lane of a CONVERGED warp, chosen by elect.sync.  The single-thread roles (TMA producer, MMA issuer) must be entered through
-// this and not through `lane == 0`: tcgen05.mma / cp.async.bulk.tensor execute on the uniform datapath, and inside a branch the
-// compiler cannot prove single-threaded it wraps EVERY such instruction in an ELECT ... BRA.U.ANY loop over the active lanes
-// (~70 cycles per MMA measured with the stamp trace of awq_decode.cu: 32 MMAs of a 256-channel block took 3 400 cycles).
+// this and not through `lane == 0`: cp.async.bulk.tensor executes on the uniform datapath, and inside a branch the compiler
+// cannot prove single-threaded it wraps EVERY such instruction in an ELECT ... BRA.U.ANY loop over the active lanes.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile(
@@ -64,78 +65,109 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* m
       ::"r"(smem_u32(smem_dst)), "l"(map), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(policy)
       : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_slot, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_slot)), "r"(cols));
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t addr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(addr), "r"(cols));
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-template <int KIND>
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  if constexpr (KIND == 0) {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n}\n"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate));
-  } else {
-    asm volatile(
-        "{\n.reg .pred p;\nsetp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n}\n"
-        ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate));
-  }
-}
-// 32 lanes x 32 columns of 32-bit accumulators -> 32 registers per thread
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-        "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-        "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr));
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-}
+// ---- wgmma (sm_90a): D[64 x N] (+)= A[64 x K] * B[N x K]^T, both operands K-major in 128B-swizzled shared memory (or A in
+// registers), accumulators in the registers of the four warps of a warpgroup ----
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): rows of 128 bytes,
-// 8-row groups 1024 bytes apart (SBO), version 1 (sm_100), layout type 2 (SWIZZLE_128B).
+// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::GmmaDescriptor): rows of 128 bytes,
+// 8-row groups 1024 bytes apart (SBO), layout type 1 (B128) in bits [62,64).
 __device__ __forceinline__ uint64_t make_smem_desc(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);        // start address, bits [0,14)
   d |= static_cast<uint64_t>(1) << 16;                           // leading byte offset (unused for SW128 K-major)
   d |= static_cast<uint64_t>(1024 >> 4) << 32;                   // stride byte offset, bits [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                           // descriptor version
-  d |= static_cast<uint64_t>(2) << 61;                           // SWIZZLE_128B
+  d |= static_cast<uint64_t>(1) << 62;                           // SWIZZLE_128B
   return d;
 }
 
-// cute::UMMA::InstrDescriptor
-template <int KIND>
-__host__ __device__ constexpr uint32_t make_idesc(int n) {
-  uint32_t d = 0;
-  d |= (KIND == 0 ? 2u : 1u) << 4;                  // c_format: S32 / F32
-  const uint32_t fmt = KIND == 0 ? 1u /*S8*/ : (KIND == 1 ? 0u /*F16*/ : 1u /*BF16*/);
-  d |= fmt << 7;                                    // a_format
-  d |= fmt << 10;                                   // b_format
-  d |= static_cast<uint32_t>(n >> 3) << 17;         // n_dim
-  d |= static_cast<uint32_t>(kTileM >> 4) << 24;    // m_dim
-  return d;                                         // a_major = b_major = K (0), dense, no negate
+#define CT2_WG_R4(d, o) "+r"(d[o]), "+r"(d[o + 1]), "+r"(d[o + 2]), "+r"(d[o + 3])
+#define CT2_WG_R8(d, o) CT2_WG_R4(d, o), CT2_WG_R4(d, o + 4)
+#define CT2_WG_R16(d, o) CT2_WG_R8(d, o), CT2_WG_R8(d, o + 8)
+#define CT2_WG_R32(d, o) CT2_WG_R16(d, o), CT2_WG_R16(d, o + 16)
+#define CT2_WG_L8 "{%0,%1,%2,%3,%4,%5,%6,%7}"
+#define CT2_WG_L16 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}"
+#define CT2_WG_L32 "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}"
+// KIND = 0 s8 (K = 32 per instruction) / 1 f16 / 2 bf16 (K = 16); acc == 0 overwrites D.  NR = N / 2 registers per thread:
+// d[4j], d[4j+1] = row 16 * warp + lane / 4, columns 8j + 2 * (lane % 4) + {0, 1};  d[4j+2], d[4j+3] = the same columns 8 rows below.
+#define CT2_WGMMA_SS(N, NR, LIST, REGS, A, B, P)                                                                                 \
+  template <int KIND>                                                                                                            \
+  __device__ __forceinline__ void wgmma_ss(uint32_t (&d)[NR], uint64_t da, uint64_t db, uint32_t acc) {                          \
+    if constexpr (KIND == 0)                                                                                                     \
+      asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, " P ", 0;\nwgmma.mma_async.sync.aligned.m64n" #N "k32.s32.s8.s8 " LIST      \
+                   ", " A ", " B ", p;\n}\n" : REGS(d, 0) : "l"(da), "l"(db), "r"(acc));                                         \
+    else if constexpr (KIND == 1)                                                                                                \
+      asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, " P ", 0;\nwgmma.mma_async.sync.aligned.m64n" #N "k16.f32.f16.f16 " LIST    \
+                   ", " A ", " B ", p, 1, 1, 0, 0;\n}\n" : REGS(d, 0) : "l"(da), "l"(db), "r"(acc));                             \
+    else                                                                                                                         \
+      asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, " P ", 0;\nwgmma.mma_async.sync.aligned.m64n" #N "k16.f32.bf16.bf16 " LIST  \
+                   ", " A ", " B ", p, 1, 1, 0, 0;\n}\n" : REGS(d, 0) : "l"(da), "l"(db), "r"(acc));                             \
+  }
+CT2_WGMMA_SS(16, 8, CT2_WG_L8, CT2_WG_R8, "%8", "%9", "%10")
+CT2_WGMMA_SS(32, 16, CT2_WG_L16, CT2_WG_R16, "%16", "%17", "%18")
+CT2_WGMMA_SS(64, 32, CT2_WG_L32, CT2_WG_R32, "%32", "%33", "%34")
+// fp16 A fragment from registers (a[0..3] = the m16n8k16 A fragment of this warp's 16 rows), B from shared memory
+#define CT2_WGMMA_RS(N, NR, LIST, REGS, A0, A1, A2, A3, B, P)                                                                    \
+  __device__ __forceinline__ void wgmma_rs_f16(uint32_t (&d)[NR], const uint32_t (&a)[4], uint64_t db, uint32_t acc) {           \
+    asm volatile("{\n.reg .pred p;\nsetp.ne.b32 p, " P ", 0;\nwgmma.mma_async.sync.aligned.m64n" #N "k16.f32.f16.f16 " LIST      \
+                 ", {" A0 "," A1 "," A2 "," A3 "}, " B ", p, 1, 1, 0;\n}\n"                                                      \
+                 : REGS(d, 0) : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(acc));                                  \
+  }
+CT2_WGMMA_RS(16, 8, CT2_WG_L8, CT2_WG_R8, "%8", "%9", "%10", "%11", "%12", "%13")
+CT2_WGMMA_RS(32, 16, CT2_WG_L16, CT2_WG_R16, "%16", "%17", "%18", "%19", "%20", "%21")
+CT2_WGMMA_RS(64, 32, CT2_WG_L32, CT2_WG_R32, "%32", "%33", "%34", "%35", "%36", "%37")
+
+// Accumulators of one 128 x BN tile in the registers of one warpgroup: [64-row half][64-column piece][wgmma D fragment]
+template <int BN> struct AccShape {
+  static_assert(BN == 16 || BN == 32 || BN % 64 == 0, "tile widths: 16, 32 or a multiple of 64");
+  static constexpr int kPiece = BN < 64 ? BN : 64;
+  static constexpr int kPieces = BN / kPiece;
+  static constexpr int kRegs = kPiece / 2;
+};
+template <int BN> struct Acc { uint32_t d[2][AccShape<BN>::kPieces][AccShape<BN>::kRegs]; };
+constexpr int kHalfTileBytes = 64 * kSwizzleBytes;      // 64 rows of a swizzled operand tile
+
+// one K block (128 bytes of K) of a 128 x BN tile: A tile at sa (128 rows), B tile at sb (BN rows); first == overwrite
+template <int KIND, int BN>
+__device__ __forceinline__ void mma_block(Acc<BN>& c, uint32_t sa, uint32_t sb, bool first) {
+  using A = AccShape<BN>;
+#pragma unroll
+  for (int k = 0; k < kSwizzleBytes / 32; ++k)          // +32 bytes of K inside the swizzle atom = +2 on the address field
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int pc = 0; pc < A::kPieces; ++pc)
+        wgmma_ss<KIND>(c.d[h][pc], make_smem_desc(sa + h * kHalfTileBytes) + 2 * k, make_smem_desc(sb + pc * kHalfTileBytes) + 2 * k,
+                       (first && k == 0) ? 0u : 1u);
+}
+
+// The fused epilogues work one output row per thread.  The warpgroup parks its fragments in shared memory as
+// [column][kAccPitch rows] (pitch 132 words: the fragment stores and the row-wise loads are both bank-conflict free).
+constexpr int kAccPitch = kTileM + 4;
+constexpr int acc_bytes(int cols) { return (cols * kAccPitch * 4 + 1023) / 1024 * 1024; }
+template <int BN>
+__device__ __forceinline__ void acc_store(const Acc<BN>& c, uint32_t* dst) {
+  using A = AccShape<BN>;
+  const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int pc = 0; pc < A::kPieces; ++pc)
+#pragma unroll
+      for (int j = 0; j < A::kPiece / 8; ++j) {
+        uint32_t* q = dst + (pc * 64 + j * 8 + (l & 3) * 2) * kAccPitch + h * 64 + w * 16 + (l >> 2);
+        q[0] = c.d[h][pc][4 * j];
+        q[kAccPitch] = c.d[h][pc][4 * j + 1];
+        q[8] = c.d[h][pc][4 * j + 2];
+        q[kAccPitch + 8] = c.d[h][pc][4 * j + 3];
+      }
+}
+// NC consecutive columns of row `rloc`
+template <int NC>
+__device__ __forceinline__ void acc_load(const uint32_t* src, int rloc, uint32_t (&r)[NC]) {
+#pragma unroll
+  for (int j = 0; j < NC; ++j) r[j] = src[j * kAccPitch + rloc];
 }
 
 

@@ -1,4 +1,4 @@
-"""`ctranslate2.Generator` for Device::CUDA on B200, on top of the C-ABI engine.
+"""`ctranslate2.Generator` for Device::CUDA on H100, on top of the C-ABI engine.
 
 Mirrors python/cpp/generator.cc:15-80 / include/ctranslate2/generator.h: `generate_batch(start_tokens, ...)`
 and `forward_batch(tokens)`.  Token strings <-> ids (ctranslate2::Vocabulary, vocabulary.json) are
@@ -296,6 +296,13 @@ class Generator:
                                          ctypes.c_int64(steps), ctypes.c_int64(warmup), ctypes.byref(pre),
                                          ctypes.byref(dec), ctypes.byref(n)))
         return pre.value, dec.value, n.value
+
+    def bench_last_logits(self, batch: int, vocab_size: int) -> np.ndarray:
+        """Logits [batch, vocab_size] float32 (host) of the last decode step bench_decode ran."""
+        out = np.empty((batch, vocab_size), np.float32)
+        check(lib().ct2b200_bench_last_logits(ctypes.c_void_p(self._h), ctypes.c_int64(batch),
+                                              out.ctypes.data_as(ctypes.POINTER(ctypes.c_float)), ctypes.c_int64(out.size)))
+        return out
 
     def info(self):
         v = [ctypes.c_int() for _ in range(5)]

@@ -1,4 +1,4 @@
-"""`ctranslate2.Translator` for Device::CUDA on B200, on top of the C-ABI engine (include/ct2b200.h, encoder-decoder path).
+"""`ctranslate2.Translator` for Device::CUDA on H100, on top of the C-ABI engine (include/ct2b200.h, encoder-decoder path).
 
 Mirrors python/cpp/translator.cc / include/ctranslate2/translator.h: `translate_batch(source, ...)` with the
 TranslationOptions of include/ctranslate2/translation.h.  Token strings <-> ids (ctranslate2::Vocabulary: source /

@@ -1,4 +1,4 @@
-"""`ctranslate2.models.Whisper` for Device::CUDA on B200, on top of the C-ABI engine (include/ct2b200.h, Whisper section).
+"""`ctranslate2.models.Whisper` for Device::CUDA on H100, on top of the C-ABI engine (include/ct2b200.h, Whisper section).
 
 Mirrors python/cpp/whisper.cc / include/ctranslate2/models/whisper.h: `encode(features)` and `generate(features, prompts, ...)`
 with the WhisperOptions of whisper.h:11-60.  Vocabulary lookups and the model's config.json (suppress_ids,

@@ -1,4 +1,4 @@
-/* ct2b200.h — C-ABI of the B200-native (sm_100a) quantized-transformer decode path.
+/* ct2b200.h — C-ABI of the H100-native (sm_90a) quantized-transformer decode path.
  *
  * This is the drop-in boundary (SURVEY.md §8b).  CTranslate2 has no C plugin interface: its
  * boundary is the set of C++ `<Device::CUDA>` template specialisations listed below.  Every entry
@@ -48,7 +48,7 @@ CT2B200_API const char* ct2b200_last_error(void);
 CT2B200_API const char* ct2b200_version(void);
 /* Number of CUDA kernels this library has launched in the calling process (all threads). */
 CT2B200_API int64_t ct2b200_kernel_launch_count(void);
-/* Device properties the host side sizes grids with; fails when there is no sm_100 device. */
+/* Device properties the host side sizes grids with; fails when there is no sm_90 device. */
 CT2B200_API int ct2b200_device_info(int device, int* sm_count, int* cc_major, int* cc_minor, size_t* total_mem);
 
 /* ---------------------------------------------------------------------------------------------
@@ -97,7 +97,7 @@ CT2B200_API int ct2b200_dense_s8_glu(const int8_t* xq_d, const float* x_scale_d,
  * ops::RMSNorm (rms_norm_gpu.cu:19-63):  xq, x_scale = Quantize([RMSNorm(x, gamma, eps)]);  y = dense_s8(xq, x_scale, ...).
  * x [m,k] T; xq_d [m,k] int8 and x_scale_d [m] are OUTPUTS (the same bits ct2b200_quantize_rows / ct2b200_rms_norm_quantize
  * produce).  Runs as the register-resident row kernel + the fused Dense under programmatic dependent launch; barrier_d is
- * unused (a variant that ran the row op inside the GEMM behind a grid barrier measured slower on the B200 and was removed). */
+ * unused. */
 CT2B200_API int ct2b200_dense_s8_rows(const void* x_d, const void* gamma_d, float eps, const int8_t* w_d, const float* w_scale_d,
                           const void* bias_d, const void* residual_d, int act, int64_t m, int64_t n, int64_t k,
                           void* y_d, int dtype, int8_t* xq_d, float* x_scale_d, unsigned* barrier_d, void* stream);
@@ -204,8 +204,8 @@ CT2B200_API int ct2b200_awq_repack(const int32_t* qweight_d, const void* scales_
                        void* stream);
 
 /* ops::GemmAwq / GemvAwq + apply_bias_and_activation — src/ops/awq/gemm.cc:8-33, gemv.cc:9-37, on the native layout:
- * y = act(x . deq(W)^T + bias) + residual.  m <= 64: fused dequantize + tcgen05 GEMM (weight-streaming kernel with the
- * operand in tensor memory when sz_d is given, the general kernel otherwise).  m > 64 (the reference's
+ * y = act(x . deq(W)^T + bias) + residual.  m <= 64: fused dequantize + wgmma GEMM (weight-streaming kernel with the
+ * operand in registers when sz_d is given, the general kernel otherwise).  m > 64 (the reference's
  * DequantizeAwq + cuBLAS arm, src/layers/common.cc:409-420): needs scratch_nk_d, an fp16 [n,k] buffer. */
 CT2B200_API int ct2b200_dense_awq(const void* x_d, const int32_t* wp_d, const void* sc_d, const void* zr_d, const void* sz_d,
                       int group_size, const void* bias_d, const void* residual_d, int act, int64_t m, int64_t n, int64_t k,
@@ -292,6 +292,10 @@ CT2B200_API int ct2b200_forward_batch(ct2b200_generator* g, const int32_t* ids_h
  * steps with inputs already resident in HBM.  Returns device milliseconds of each phase. */
 CT2B200_API int ct2b200_bench_decode(ct2b200_generator* g, int64_t batch, int64_t prompt_len, int64_t steps, int64_t warmup,
                          float* prefill_ms, float* decode_ms, int64_t* kernel_launches);
+
+/* The logits of the last decode step ct2b200_bench_decode ran: logits_h [batch, vocab] f32 host, of logits_len floats
+ * (an error unless logits_len == batch * vocab of the model). */
+CT2B200_API int ct2b200_bench_last_logits(ct2b200_generator* g, int64_t batch, float* logits_h, int64_t logits_len);
 
 /* Tensor parallel (ct2b200_generator_config.tp_size > 1; one process per GPU; replaces ScopedMPISetter + the NCCL
  * communicator of src/devices.cc:141-217 and ops::ReduceAll / GatherAll, src/ops/nccl_ops_gpu.cu:52-85).

@@ -3,7 +3,7 @@
 // specialisation the reference links today (file:line cited), re-implemented as a call into the C-ABI of include/ct2b200.h.
 // Built as its own shared library (oracle/Makefile.shims) and placed in front of the reference's CUDA build, it interposes
 // those symbols: the reference's own device-parameterised gtests (tests/ops_test.cc, primitives_test.cc, layers_test.cc) then
-// run with the B200 kernels underneath.  Forms the C-ABI does not cover (an axis other than the last, non-transposed rotary
+// run with the H100 kernels underneath.  Forms the C-ABI does not cover (an axis other than the last, non-transposed rotary
 // layouts, ...) are forwarded to the reference's own implementation (dlsym(RTLD_NEXT)), and every call is counted so the
 // run reports how many went where.  TEST / INTEGRATION INFRASTRUCTURE: nothing in ctranslate2_b200/ depends on this file.
 #include <dlfcn.h>

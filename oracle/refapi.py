@@ -1,6 +1,6 @@
 """ctypes binding of oracle/_ref/libct2ref_driver.so (the UNMODIFIED reference, CPU build) and of
 oracle/_ref_cuda/libct2ref_cuda_driver.so (the UNMODIFIED reference WITH its CUDA backend: cuBLAS GEMM,
-its own AWQ / FlashAttention-2 kernels, compiled for sm_100 by oracle/Makefile.ref_cuda).
+its own AWQ / FlashAttention-2 kernels, compiled for sm_90 by oracle/Makefile.ref_cuda).
 
 TEST INFRASTRUCTURE: only tests/, tools/make_golden*.py, __graft_entry__.smoke() and bench.py's
 reference legs import this.  `available()` / `cuda_available()` are False when the library was not built

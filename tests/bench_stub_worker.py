@@ -44,6 +44,10 @@ class FakeGenerator:
             time.sleep(3600)                     # a peer-flag wait that never ends
         return 280.0, (2.7 if self.tp else 3.0) * steps, 292 * steps
 
+    def bench_last_logits(self, batch, vocab_size):
+        import numpy as np
+        return np.full((batch, vocab_size), 0.5, np.float32)
+
     def generate_batch(self, prompts, max_length=1, **kw):
         return [_Result(max_length) for _ in range(len(prompts))]
 

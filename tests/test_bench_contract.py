@@ -137,3 +137,19 @@ def test_tp_record_failure_keeps_the_replica_line(mode):
     assert len(lines) == 1, r.stdout + r.stderr[-1500:]
     d = json.loads(lines[0])
     assert d["n_gpus"] == 2 and d["value"] > 0 and "error" in d["tp"], d.get("tp")
+
+
+@pytest.mark.timeout(300)
+def test_dump_outputs_writes_the_last_step_logits(tmp_path):
+    """`--dump-outputs DIR` (device layer stubbed): DIR/logits.npy holds what the last timed step computed, [batch, vocab]
+    float32 within 64 MB, beside the unchanged result line; the reference arm refuses the flag instead of ignoring it."""
+    import numpy as np
+    out = tmp_path / "dump"
+    r, lines = _run_stub(1, extra=("--no-variants", "--no-cpu-baseline", "--dump-outputs", str(out)))
+    assert r.returncode == 0, r.stderr[-2000:]
+    assert len(lines) == 1 and json.loads(lines[0])["steps"] == 8
+    assert sorted(os.listdir(out)) == ["logits.npy"]
+    a = np.load(out / "logits.npy")
+    assert a.dtype == np.float32 and a.shape == (32, 128256) and a.nbytes <= 64 << 20 and (a == 0.5).all()
+    r, lines = _run_stub(1, extra=("--impl", "reference", "--dump-outputs", str(tmp_path / "none")))
+    assert r.returncode != 0 and not lines and not os.path.exists(tmp_path / "none")

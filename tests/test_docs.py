@@ -29,7 +29,7 @@ def test_every_environment_switch_is_documented_in_the_readme():
 
 def test_design_and_integration_cite_existing_files():
     """Paths of this repository named in DESIGN.md / INTEGRATION.md / README.md exist."""
-    pat = re.compile(r"`((?:ctranslate2_b200|oracle|tests|tools|profiles|include)/[A-Za-z0-9_./-]+\.(?:cu|cuh|cc|h|py|md|sh|json|csv))`")
-    for doc in ("DESIGN.md", "INTEGRATION.md", "README.md", os.path.join("profiles", "README.md")):
+    pat = re.compile(r"`((?:ctranslate2_b200|oracle|tests|tools|include)/[A-Za-z0-9_./-]+\.(?:cu|cuh|cc|h|py|md|sh|json|csv))`")
+    for doc in ("DESIGN.md", "INTEGRATION.md", "README.md"):
         for path in pat.findall(_read(doc)):
             assert os.path.exists(os.path.join(ROOT, path)), "%s cites a missing file: %s" % (doc, path)

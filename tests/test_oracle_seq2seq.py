@@ -1,8 +1,8 @@
 """Encoder-decoder restatement (SURVEY §8 f1: Translator::translate_batch) pinned against the unmodified reference.
 
 The golden case is the reference's own tests/translator_test.cc:53-96 (aren-transliteration-i8: "آ ت ز م و ن" ->
-"a t z m o n").  The model file lives under /root/reference, so these run where the reference tree is mounted (the CPU
-suite in the build container) and skip elsewhere.  Nothing here touches the product.
+"a t z m o n"), on the committed copy of its model (tests/golden/aren-transliteration-i8).  They run where the reference has
+been compiled (oracle/_ref) and skip elsewhere.  Nothing here touches the product.
 """
 import os
 import struct
@@ -13,9 +13,8 @@ import pytest
 from oracle import ct2_oracle as O
 from oracle import refapi
 
-MODEL = "/root/reference/tests/data/models/v2/aren-transliteration-i8"
-needs_reference = pytest.mark.skipif(not (refapi.available() and os.path.isdir(MODEL)),
-                                     reason="needs oracle/_ref and the reference's test model")
+MODEL = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "aren-transliteration-i8")
+needs_reference = pytest.mark.skipif(not refapi.available(), reason="needs oracle/_ref")
 
 
 def _vocab(name):

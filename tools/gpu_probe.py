@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""First-contact probe for a fresh B200 box: exercises each kernel family once with diagnostics
+"""First-contact probe for a fresh H100 box: exercises each kernel family once with diagnostics
 (prints what differs instead of just failing).  Usage: python tools/gpu_probe.py [tc|mma|attn|engine|all]"""
 import os
 import sys
@@ -42,7 +42,7 @@ def probe_gemm(impl, name):
 
 
 def probe_f16():
-    print("== f16/bf16 GEMM (tcgen05)")
+    print("== f16/bf16 GEMM (wgmma)")
     for dt in (torch.float16, torch.bfloat16):
         for (m, n, k) in [(128, 256, 64), (8, 512, 1024), (300, 640, 512)]:
             a = torch.randn((m, k), device="cuda").to(dt)

@@ -5,6 +5,7 @@ oracle and the `ref_cuda` performance record; nothing under ctranslate2_b200/ im
 
     python tools/ref_cuda_worker.py awq-golden OUT.npz            # GemmAwq / GemvAwq / DequantizeAwq outputs on seeded inputs
     python tools/ref_cuda_worker.py dense-s8 OUT.npz              # Quantize + cublasGemmEx(s8) + Dequantize on seeded inputs
+    python tools/ref_cuda_worker.py model-golden OUT_DIR          # full-size Llama-3-8B INT8 logits / tokens, OPUS-shaped translations
     python tools/ref_cuda_worker.py forward MODEL_DIR COMPUTE IDS.npy OUT.npy [--flash]
     python tools/ref_cuda_worker.py generate MODEL_DIR COMPUTE PROMPTS.npy MAXLEN OUT.npy [--flash]
     python tools/ref_cuda_worker.py bench MODEL_DIR COMPUTE BATCH PROMPT_LEN G1 G2 [--flash]   # one JSON line
@@ -31,7 +32,7 @@ from oracle import refapi            # noqa: E402
 AWQ_GEMM, AWQ_GEMV = 1, 2
 # (m, n, k, g, seed): m <= 8 takes the reference's gemv kernel, m > 8 its gemv2 (split-K + Sum); GemmAwq covers all m
 # (k / g >= 8 everywhere: the reference's gemv kernels read whole 32-bit words of 8 zero points per row, gemv_gpu.cu:305-307,
-# 380-382; with fewer groups than that — k = 512, g = 128 — its own output is garbage / NaN, measured on the B200)
+# 380-382; with fewer groups than that — k = 512, g = 128 — its own output is garbage / NaN)
 AWQ_CASES = [(1, 256, 1024, 128, 11), (4, 256, 2048, 128, 12), (8, 384, 1024, 64, 13), (16, 256, 1024, 128, 14),
              (40, 384, 1024, 64, 15), (7, 1024, 4096, 128, 16), (32, 1024, 4096, 128, 17)]
 DEQ_CASES = [(256, 512, 128, 21), (384, 1024, 64, 22)]
@@ -96,6 +97,49 @@ def dense_s8(out):
     np.savez_compressed(out, **res)
 
 
+# ---- whole-model fixtures (tests/golden/llama8b_int8_ref_cuda.npz, opus_small_ref_cuda.json): seeded inputs shared with
+# tests/test_gpu_ref_cuda.py, which compares against what `model-golden` stored ----
+LLAMA_VOCAB = 128256
+LLAMA_SAMPLE_COLS = 512          # vocabulary columns of the reference logits that are stored (all 128256 would be 25 MB)
+LLAMA_TOP = 8                    # plus the reference's top entries of every position (argmax and margin are exact)
+
+
+def llama8b_inputs():
+    r = np.random.default_rng(7)
+    ids = r.integers(3, LLAMA_VOCAB, size=(2, 24)).astype(np.int32)
+    prompts = r.integers(3, LLAMA_VOCAB, size=(4, 48)).astype(np.int32)
+    cols = np.sort(np.random.default_rng(70).choice(LLAMA_VOCAB, LLAMA_SAMPLE_COLS, replace=False))
+    return ids, prompts, cols
+
+
+def opus_small(model_dir):
+    """BASELINE.json configs[1] geometry with the vocabulary cut to 4000; returns the 16 source sentences."""
+    from ctranslate2_b200.converters.synthetic import TransformerConfig, write_transformer_model
+    cfg = TransformerConfig(source_vocab=4000, target_vocab=4000, pre_norm=False, activation=2, start_from_zero_embedding=True)
+    write_transformer_model(model_dir, cfg, "int8", seed=3)
+    r = np.random.default_rng(11)
+    return [[int(x) for x in r.integers(3, 4000, size=int(r.integers(10, 50)))] for _ in range(16)]
+
+
+def model_golden(out_dir):
+    import tempfile
+    import bench
+    ids, prompts, cols = llama8b_inputs()
+    g = open_generator(bench.model_dir("8b"), "int8_float16")
+    logits = g.forward(ids)                                            # [2, 24, V] fp32
+    top_idx = np.argsort(-logits, axis=-1, kind="stable")[..., :LLAMA_TOP].astype(np.int32)
+    tokens, _ = g.generate_timed(prompts, 8, end_id=2)
+    np.savez_compressed(os.path.join(out_dir, "llama8b_int8_ref_cuda.npz"), logits_cols=logits[..., cols].astype(np.float32),
+                        top_idx=top_idx, top_val=np.take_along_axis(logits, top_idx, -1).astype(np.float32),
+                        tokens=np.asarray(tokens, np.int32))
+    del g
+    with tempfile.TemporaryDirectory() as tmp:
+        srcs = opus_small(os.path.join(tmp, "opus_small"))
+        t = refapi.RefTranslator(os.path.join(tmp, "opus_small"), "float32", 0)
+        res = t.translate(srcs, beam_size=4, num_hypotheses=2, max_length=24)
+    json.dump([[[h[0], h[1]] for h in r] for r in res], open(os.path.join(out_dir, "opus_small_ref_cuda.json"), "w"))
+
+
 def open_generator(model_dir, compute):
     return refapi.RefGenerator(model_dir, compute, 0)
 
@@ -112,6 +156,8 @@ def main():
         awq_golden(args[1])
     elif task == "dense-s8":
         dense_s8(args[1])
+    elif task == "model-golden":
+        model_golden(args[1])
     elif task == "forward":
         g = open_generator(args[1], args[2])
         ids = np.load(args[3]).astype(np.int32)
