@@ -134,13 +134,11 @@ void rows_to_int8(const void* x, const void* gamma, float eps, int64_t m, int64_
 
 CT2B200_API int ct2b200_dense_s8_rows(const void* x, const void* gamma, float eps, const int8_t* w, const float* w_scale,
                           const void* bias, const void* residual, int act, int64_t m, int64_t n, int64_t k, void* y,
-                          int dtype, int8_t* xq, float* x_scale, unsigned* barrier, void* stream) {
+                          int dtype, int8_t* xq, float* x_scale, void* stream) {
   return guarded([&] {
     require_device();
-    CT2_REQUIRE(x && w && w_scale && xq && x_scale && barrier, "dense_s8_rows: null argument");
+    CT2_REQUIRE(x && w && w_scale && xq && x_scale, "dense_s8_rows: null argument");
     DenseEpilogue e{x_scale, w_scale, bias, residual, y, nullptr, act, n};
-    RowPre pre{gamma ? 2 : 1, x, gamma, eps, barrier};
-    if (m <= 64 && gemm_s8_decode(xq, w, m, n, k, e, dtype, S(stream), &pre)) return;
     rows_to_int8(x, gamma, eps, m, k, dtype, xq, x_scale, S(stream));
     gemm_s8(xq, w, m, n, k, e, dtype, CT2B200_GEMM_AUTO, S(stream));
   });
@@ -148,14 +146,11 @@ CT2B200_API int ct2b200_dense_s8_rows(const void* x, const void* gamma, float ep
 
 CT2B200_API int ct2b200_dense_s8_glu_rows(const void* x, const void* gamma, float eps, const int8_t* w_gate,
                               const float* w_gate_scale, const int8_t* w_up, const float* w_up_scale, int act, int64_t m,
-                              int64_t n, int64_t k, void* h, int dtype, int8_t* xq, float* x_scale, unsigned* barrier,
-                              void* stream) {
+                              int64_t n, int64_t k, void* h, int dtype, int8_t* xq, float* x_scale, void* stream) {
   return guarded([&] {
     require_device();
-    CT2_REQUIRE(x && w_gate && w_up && xq && x_scale && barrier, "dense_s8_glu_rows: null argument");
+    CT2_REQUIRE(x && w_gate && w_up && xq && x_scale, "dense_s8_glu_rows: null argument");
     GluEpilogue g{x_scale, w_gate_scale, w_up_scale, h, act, n};
-    RowPre pre{gamma ? 2 : 1, x, gamma, eps, barrier};
-    if (m <= 64 && gemm_s8_glu_decode(xq, w_gate, w_up, m, n, k, g, dtype, S(stream), &pre)) return;
     rows_to_int8(x, gamma, eps, m, k, dtype, xq, x_scale, S(stream));
     gemm_s8_glu(xq, w_gate, w_up, m, n, k, g, dtype, CT2B200_GEMM_AUTO, S(stream));
   });

@@ -185,20 +185,38 @@ void allow_dynamic_smem(K kernel, size_t bytes) {
     CT2_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(bytes)));
 }
 
+// One launch with the attributes the kernels use: a thread-block cluster of `cs` CTAs when cs > 1, programmatic dependent
+// launch when enabled.
 template <typename... KArgs, typename... Args>
-void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
-  if (mark_configured(reinterpret_cast<const void*>(kernel))) prefer_max_shared(kernel);
+void launch_clustered(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, int cs, cudaStream_t st, Args&&... args) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid;
   cfg.blockDim = block;
   cfg.dynamicSmemBytes = smem;
   cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cudaLaunchAttribute attr[2];
+  int na = 0;
+  if (cs > 1) {
+    attr[na].id = cudaLaunchAttributeClusterDimension;
+    attr[na].val.clusterDim.x = cs;
+    attr[na].val.clusterDim.y = 1;
+    attr[na].val.clusterDim.z = 1;
+    ++na;
+  }
+  if (pdl_enabled()) {
+    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[na].val.programmaticStreamSerializationAllowed = 1;
+    ++na;
+  }
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = na;
   CT2_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, KArgs(std::forward<Args>(args))...));
+}
+
+template <typename... KArgs, typename... Args>
+void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+  if (mark_configured(reinterpret_cast<const void*>(kernel))) prefer_max_shared(kernel);
+  launch_clustered(kernel, grid, block, smem, 1, st, std::forward<Args>(args)...);
 }
 
 inline int div_up(int64_t a, int64_t b) { return static_cast<int>((a + b - 1) / b); }

@@ -17,10 +17,6 @@
 //     sub.f16x2 + fma.rn.f16x2): in the native word layout the pair (k 2t, k 2t + 1) of a word is one lop3 away.
 //   * wgmma f16 with A from registers, B (activations) from 128B-swizzled smem, fp32 accumulators in registers;
 //     epilogue = gemm_decode_common.cuh (float arm).
-#include <map>
-#include <mutex>
-#include <tuple>
-
 #include "awq_common.cuh"
 #include "gemm_decode_common.cuh"
 #include "kernels.h"
@@ -41,10 +37,8 @@ constexpr int kPairs = kSub * kPairBytes;       // up to 4 groups per slot (grou
 constexpr int kMaxP = 8;
 
 struct AwqDecParams {
-  DecParams d;
-  int64_t k;
+  DecParams d;                   // d.stages = depth of the packed / pairs / activation ring
   int group;
-  int p_stages;                  // depth of the packed / pairs / activation ring
   int sb_total;                  // super-blocks (256 channels) along K
   const __half2* sz[2];          // {scale, zero} [k/group, n] (group-major): 512 contiguous bytes per tile and group
 };
@@ -55,9 +49,8 @@ struct AwqDecSmem {
   static constexpr int kP = NB * (kPacked + kPairs) + kSub * kAct;          // one ring slot: nibbles | pairs | 4 activation atoms
   static constexpr int kCtrl = 1024;
   static constexpr int kAcc = acc_bytes(NB * BN);                           // accumulators parked for the row-per-thread epilogue
-  static size_t red_bytes(int cs) { return cs > 1 ? static_cast<size_t>(cs) * NB * (BN / 16) * ((16 + cs - 1) / cs) * kTileM * 4 : 0; }
   static size_t bytes(int p_stages, int cs) {
-    return kAcc + static_cast<size_t>(p_stages) * kP + kCtrl + red_bytes(cs) + 1024;
+    return kAcc + static_cast<size_t>(p_stages) * kP + kCtrl + red_bytes(cs, NB, BN) + 1024;
   }
 };
 
@@ -81,20 +74,17 @@ __global__ void __launch_bounds__(kThreads, 1)
     awq_decode_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w,
                       const __grid_constant__ CUtensorMap tm_w2, const AwqDecParams ap) {
   using S = AwqDecSmem<BN, NB>;
-  using T = __half;
   const DecParams& p = ap.d;
-  constexpr int cp16 = (16 + CS - 1) / CS;
-  constexpr int cpr = (BN / 16) * cp16;
 
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint32_t* accs = reinterpret_cast<uint32_t*>(smem);             // [NB * BN columns][kAccPitch]
   uint8_t* p_ring = smem + S::kAcc;                               // [p_stages][nibbles NB x 16 KB | pairs NB x 2 KB | x 4 x BN x 128 B]
-  const int PD = ap.p_stages;
+  const int PD = p.stages;
   uint8_t* ctrl = p_ring + static_cast<size_t>(PD) * S::kP;
   uint64_t* p_full = reinterpret_cast<uint64_t*>(ctrl);           // [kMaxP] TMA landed
   uint64_t* p_free = p_full + kMaxP;                              // [kMaxP] the consumer warps are done with the slot
-  uint32_t* red = reinterpret_cast<uint32_t*>(ctrl + S::kCtrl);
+  uint32_t* red = reinterpret_cast<uint32_t*>(ctrl + S::kCtrl);   // split-K exchange buffer (CS > 1)
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int tile = blockIdx.x / CS;
@@ -104,17 +94,7 @@ __global__ void __launch_bounds__(kThreads, 1)
   const int a0 = tile * p.tile_rows;
   const int ngs = max(1, kSlotK / ap.group);                       // distinct groups inside a super-block (group >= 64)
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < PD; ++s) {
-      mbar_init(p_full + s, 1);
-      mbar_init(p_free + s, 4);                                    // one arrive per consumer warp
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  __syncthreads();
-  griddep_launch();
-  if (CS > 1) cluster_arrive();
+  ring_init<CS>(p_full, p_free, PD);
 
   if (warp == kProducerWarp) {
     // ===== TMA producer: packed nibbles, {scale, zero} pairs (both weights are constants: issued before the grid
@@ -138,160 +118,68 @@ __global__ void __launch_bounds__(kThreads, 1)
 #pragma unroll
         for (int j = 0; j < kSub; ++j) tma_load_2d(at + j * S::kAct, &tm_x, p_full + s, (sb * kSub + j) * kBKh, 0, kEvictLast);
       };
-      const int pre = min(PD, nsb);
-#pragma unroll 1
-      for (int i = 0; i < pre; ++i) {
-        mbar_expect_tx(p_full + i, tx);
-        weights(i, sb_lo + i);
-      }
-      griddep_wait();
-#pragma unroll 1
-      for (int i = 0; i < pre; ++i) acts(i, sb_lo + i);
-#pragma unroll 1
-      for (int it = pre; it < nsb; ++it) {
-        const int s = it % PD;
-        mbar_wait(p_free + s, ((it / PD) & 1) ^ 1);
-        mbar_expect_tx(p_full + s, tx);
-        weights(s, sb_lo + it);
-        acts(s, sb_lo + it);
-      }
+      produce(p_full, p_free, PD, tx, sb_lo, nsb, weights, acts);
     }
+    split_k_epilogue<__half, 1, BN, NB, CS, false>(p, accs, red, a0, crank);
   } else {
-    // ===== consumer warpgroup: nibbles -> fp16 A fragments in registers -> wgmma; then thread = output channel =====
+    // ===== consumer warpgroup: nibbles -> fp16 A fragments in registers -> wgmma =====
     const int q = warp & 3;
-    const int rloc = q * 32 + lane;
-    const int64_t arow = static_cast<int64_t>(a0) + rloc;
-    const bool row_ok = rloc < p.tile_rows && arow < p.n;
-    {
-      const int t = lane & 3;                                      // channel pair of the A fragment held by this thread
-      const uint32_t shift = (t & 2) ? 8u : 0u, mask = (t & 1) ? 0x00f000f0u : 0x000f000fu;
-      const __half2 mul = __float2half2_rn((t & 1) ? 0.0625f : 1.f);
-      Acc<BN> acc[NB];
+    const int t = lane & 3;                                      // channel pair of the A fragment held by this thread
+    const uint32_t shift = (t & 2) ? 8u : 0u, mask = (t & 1) ? 0x00f000f0u : 0x000f000fu;
+    const __half2 mul = __float2half2_rn((t & 1) ? 0.0625f : 1.f);
+    Acc<BN> acc[NB];
 #pragma unroll 1
-      for (int sb = 0; sb < nsb; ++sb) {
-        const int sp = sb % PD;
-        mbar_wait(p_full + sp, (sb / PD) & 1);
-        const uint8_t* pk = p_ring + static_cast<size_t>(sp) * S::kP;
-        const uint32_t act0 = smem_u32(pk + NB * (kPacked + kPairs));
+    for (int sb = 0; sb < nsb; ++sb) {
+      const int sp = sb % PD;
+      mbar_wait(p_full + sp, (sb / PD) & 1);
+      const uint8_t* pk = p_ring + static_cast<size_t>(sp) * S::kP;
+      const uint32_t act0 = smem_u32(pk + NB * (kPacked + kPairs));
 #pragma unroll 1
-        for (int j = 0; j < kSub; ++j) {                           // K block j of the slot: 32 bytes of every packed row
-          const int pair_slot = (j * kBKh) / ap.group < ngs ? (j * kBKh) / ap.group : ngs - 1;
-          const uint64_t db = make_smem_desc(act0 + j * S::kAct);
-#pragma unroll
-          for (int w = 0; w < NB; ++w)
-#pragma unroll
-            for (int h = 0; h < 2; ++h) {
-              uint32_t a[kBKh / 16][4];
-#pragma unroll
-              for (int rr = 0; rr < 2; ++rr) {                     // rows g, g + 8 of this warp's 16
-                const int r = h * 64 + q * 16 + (lane >> 2) + rr * 8;
-                const __half2 sz = *reinterpret_cast<const __half2*>(pk + NB * kPacked + w * kPairs + pair_slot * kPairBytes + r * 4);
-                const __half zp = __high2half(sz);
-                const __half2 add = __half2half2((t & 1) ? __hneg(__hadd(__float2half(64.f), zp)) : __hneg(__hadd(__float2half(1024.f), zp)));
-                const __half2 s2 = __half2half2(__low2half(sz));
-                // the 16-byte chunks 2j, 2j + 1 of the row's 128 bytes are stored at chunk ^ (r % 8) by the 128-byte swizzle
-                const uint8_t* row = pk + w * kPacked + r * kSwizzleBytes;
-                const uint4 w0 = *reinterpret_cast<const uint4*>(row + (((2 * j) ^ (r & 7)) << 4));
-                const uint4 w1 = *reinterpret_cast<const uint4*>(row + (((2 * j + 1) ^ (r & 7)) << 4));
-                const uint32_t words[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
-#pragma unroll
-                for (int k = 0; k < kBKh / 16; ++k) {              // word 2k = channels 16k .. 16k+7, word 2k+1 = 16k+8 .. 16k+15
-                  a[k][rr] = awq_dequant_pair(words[2 * k], shift, mask, mul, add, s2);
-                  a[k][2 + rr] = awq_dequant_pair(words[2 * k + 1], shift, mask, mul, add, s2);
-                }
-              }
-              wgmma_fence();
-#pragma unroll
-              for (int k = 0; k < kBKh / 16; ++k)
-                wgmma_rs_f16(acc[w].d[h][0], a[k], db + 2 * k, (sb == 0 && j == 0 && k == 0) ? 0u : 1u);
-              wgmma_commit();
-              wgmma_wait();                                        // the A registers are rewritten by the next conversion
-            }
-        }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(p_free + sp);
-      }
-#pragma unroll
-      for (int w = 0; w < NB; ++w) acc_store<BN>(acc[w], accs + w * BN * kAccPitch);
-      epi_bar_sync();
-    }
-    griddep_wait();
-    float bias_t = 0.f;
-    if (row_ok && p.bias) bias_t = to_f32(static_cast<const T*>(p.bias)[arow]);
-    auto load_acc = [&](int c0, uint32_t (&r)[NB][16]) {
-#pragma unroll
-      for (int w = 0; w < NB; ++w) acc_load<16>(accs + (w * BN + c0) * kAccPitch, rloc, r[w]);
-    };
-    if constexpr (CS == 1) {
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 16) {
-        uint32_t r[NB][16];
-        load_acc(c0, r);
-        if (row_ok && c0 < p.m) dec_finish<T, 1, NB, 16>(p, r, arow, c0, 1, 16, 1.f, 1.f, bias_t);
-      }
-    } else {
-      cluster_wait();
-      uint32_t peer[CS];
-#pragma unroll
-      for (int o = 0; o < CS; ++o) {
-        const uint32_t local = smem_u32(red + static_cast<size_t>(crank) * NB * cpr * kTileM + rloc);
-        asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(peer[o]) : "r"(local), "r"(o));
-      }
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 16) {
-        uint32_t r[NB][16];
-        load_acc(c0, r);
-        const uint32_t chunk_off = static_cast<uint32_t>((c0 / 16) * cp16 * kTileM * 4);
-#pragma unroll
-        for (int j = 0; j < 16; ++j)
-#pragma unroll
-          for (int w = 0; w < NB; ++w) {
-            const uint32_t off = static_cast<uint32_t>((w * cpr + j / CS) * kTileM * 4);
-            asm volatile("st.shared::cluster.u32 [%0], %1;" ::"r"(peer[j % CS] + chunk_off + off), "r"(r[w][j]) : "memory");
-          }
-      }
-    }
-  }
-
-  if constexpr (CS > 1) {
-    __syncwarp();
-    if (warp == kProducerWarp) cluster_wait();         // phase 1 (the consumer warps consumed it above)
-    cluster_arrive();
-    cluster_wait();
-    if (warp < kProducerWarp) {
-      const int q = warp & 3;
-      const int rloc = q * 32 + lane;
-      const int64_t arow = static_cast<int64_t>(a0) + rloc;
-      const bool row_ok = rloc < p.tile_rows && arow < p.n;
-      float bias_t = 0.f;
-      if (row_ok && p.bias) bias_t = to_f32(static_cast<const T*>(p.bias)[arow]);
-      const int nvalid = (16 - crank + CS - 1) / CS;
-#pragma unroll 1
-      for (int ch = 0; ch < BN / 16; ++ch) {
-        uint32_t r[NB][cp16];
+      for (int j = 0; j < kSub; ++j) {                           // K block j of the slot: 32 bytes of every packed row
+        const int pair_slot = (j * kBKh) / ap.group < ngs ? (j * kBKh) / ap.group : ngs - 1;
+        const uint64_t db = make_smem_desc(act0 + j * S::kAct);
 #pragma unroll
         for (int w = 0; w < NB; ++w)
 #pragma unroll
-          for (int jj = 0; jj < cp16; ++jj) {
-            float acc = 0.f;
+          for (int h = 0; h < 2; ++h) {
+            uint32_t a[kBKh / 16][4];
 #pragma unroll
-            for (int src = 0; src < CS; ++src)         // fixed rank order: deterministic
-              acc += __uint_as_float(red[(static_cast<size_t>(src * NB + w) * cpr + ch * cp16 + jj) * kTileM + rloc]);
-            r[w][jj] = __float_as_uint(acc);
+            for (int rr = 0; rr < 2; ++rr) {                     // rows g, g + 8 of this warp's 16
+              const int r = h * 64 + q * 16 + (lane >> 2) + rr * 8;
+              const __half2 sz = *reinterpret_cast<const __half2*>(pk + NB * kPacked + w * kPairs + pair_slot * kPairBytes + r * 4);
+              const __half zp = __high2half(sz);
+              const __half2 add = __half2half2((t & 1) ? __hneg(__hadd(__float2half(64.f), zp)) : __hneg(__hadd(__float2half(1024.f), zp)));
+              const __half2 s2 = __half2half2(__low2half(sz));
+              // the 16-byte chunks 2j, 2j + 1 of the row's 128 bytes are stored at chunk ^ (r % 8) by the 128-byte swizzle
+              const uint8_t* row = pk + w * kPacked + r * kSwizzleBytes;
+              const uint4 w0 = *reinterpret_cast<const uint4*>(row + (((2 * j) ^ (r & 7)) << 4));
+              const uint4 w1 = *reinterpret_cast<const uint4*>(row + (((2 * j + 1) ^ (r & 7)) << 4));
+              const uint32_t words[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+#pragma unroll
+              for (int k = 0; k < kBKh / 16; ++k) {              // word 2k = channels 16k .. 16k+7, word 2k+1 = 16k+8 .. 16k+15
+                a[k][rr] = awq_dequant_pair(words[2 * k], shift, mask, mul, add, s2);
+                a[k][2 + rr] = awq_dequant_pair(words[2 * k + 1], shift, mask, mul, add, s2);
+              }
+            }
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < kBKh / 16; ++k)
+              wgmma_rs_f16(acc[w].d[h][0], a[k], db + 2 * k, (sb == 0 && j == 0 && k == 0) ? 0u : 1u);
+            wgmma_commit();
+            wgmma_wait();                                        // the A registers are rewritten by the next conversion
           }
-        const int col0 = ch * 16 + crank;
-        if (row_ok && col0 < p.m) dec_finish<T, 1, NB, cp16>(p, r, arow, col0, CS, nvalid, 1.f, 1.f, bias_t);
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(p_free + sp);
     }
+#pragma unroll
+    for (int w = 0; w < NB; ++w) acc_store<BN>(acc[w], accs + w * BN * kAccPitch);
+    epi_bar_sync();
+    split_k_epilogue<__half, 1, BN, NB, CS, true>(p, accs, red, a0, crank);   // float arm: fp32 partials, no scales
   }
-
 }
 
 // ---- host side ----
-struct AwqPlan {
-  int cs = 0, tile_rows = 128, tiles = 0, p_stages = 4;
-};
-
 CUtensorMap make_packed_map(const void* wp, int64_t n, int64_t k, int box_rows) {
   // wp as bytes [n, k/2]; box = box_rows x 128 bytes (a super-block of 256 channels), 128-byte swizzle
   CUtensorMap m;
@@ -310,48 +198,16 @@ template <int BN, int NB>
 int p_stages_for(int cs, int nkb) {
   using S = AwqDecSmem<BN, NB>;
   const size_t cap = 220 * 1024;
-  const size_t fixed = S::kAcc + S::kCtrl + S::red_bytes(cs) + 1024;
+  const size_t fixed = S::kAcc + S::kCtrl + red_bytes(cs, NB, BN) + 1024;
   if (fixed + 2 * S::kP > cap) return 0;
   int st = static_cast<int>((cap - fixed) / S::kP);
   st = std::min(st, kMaxP);
   return std::max(2, std::min(st, std::max(nkb, 2)));
 }
 
-template <int BN, int NB, int CS>
-void configure_once() {
-  allow_dynamic_smem(awq_decode_kernel<BN, NB, CS>, 226 * 1024);
-}
-
-template <int BN, int NB, int CS>
-int clusters_for(int p_stages, int sm_count) {
-  configure_once<BN, NB, CS>();
-  static std::mutex mu;
-  static std::map<std::pair<int, int>, int> cache;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  std::lock_guard<std::mutex> lock(mu);
-  auto it = cache.find({dev, p_stages});
-  if (it != cache.end()) return it->second;
-  const int n = max_clusters(awq_decode_kernel<BN, NB, CS>, CS, kThreads, AwqDecSmem<BN, NB>::bytes(p_stages, CS), sm_count);
-  cache[{dev, p_stages}] = n;
-  return n;
-}
-
 template <int BN, int NB>
-AwqPlan plan_awq(int64_t n, int kb_total /* super-blocks */, int sm_count) {
-  static std::mutex mu;
-  static std::map<std::tuple<int, int64_t, int>, AwqPlan> cache;
-  int dev = 0;
-  cudaGetDevice(&dev);
-  const int force_cs = env_int("CT2B200_GEMM_CS", 0);
-  const int force_rows = env_int("CT2B200_GEMM_ROWS", 0);
-  const bool forced = force_cs != 0 || force_rows != 0;
-  if (!forced) {
-    std::lock_guard<std::mutex> lock(mu);
-    auto it = cache.find({dev, n, kb_total});
-    if (it != cache.end()) return it->second;
-  }
-  AwqPlan best;
+Plan plan_awq(int64_t n, int kb_total /* super-blocks */, int sm_count, int force_cs, int force_rows) {
+  Plan best;
   double best_cost = 1e30;
   for (int cs = 1; cs <= 4; ++cs) {
     if (force_cs && cs != force_cs) continue;
@@ -359,13 +215,9 @@ AwqPlan plan_awq(int64_t n, int kb_total /* super-blocks */, int sm_count) {
     const int nkb = (kb_total + cs - 1) / cs;
     const int ps = p_stages_for<BN, NB>(cs, nkb);
     if (ps == 0) continue;
-    int maxc = 0;
-    switch (cs) {
-      case 1: maxc = clusters_for<BN, NB, 1>(ps, sm_count); break;
-      case 2: maxc = clusters_for<BN, NB, 2>(ps, sm_count); break;
-      case 3: maxc = clusters_for<BN, NB, 3>(ps, sm_count); break;
-      default: maxc = clusters_for<BN, NB, 4>(ps, sm_count); break;
-    }
+    const int maxc = dispatch_cs(cs, [&](auto c) {
+      return max_clusters(awq_decode_kernel<BN, NB, decltype(c)::value>, cs, kThreads, AwqDecSmem<BN, NB>::bytes(ps, cs), sm_count);
+    });
     // Tile height.  The conversion covers all 128 rows of a block whatever the tile height, so full-height tiles waste nothing;
     // a shorter tile that puts the stream on more SMs wins when 128-row tiles leave many idle.
     // cost = streamed rows x K blocks per CTA (+ the cluster exchange).
@@ -385,71 +237,39 @@ AwqPlan plan_awq(int64_t n, int kb_total /* super-blocks */, int sm_count) {
         best.cs = cs;
         best.tile_rows = rows;
         best.tiles = tiles;
-        best.p_stages = ps;
+        best.stages = ps;
       }
     }
   }
-  if (!forced) {
-    std::lock_guard<std::mutex> lock(mu);
-    cache[{dev, n, kb_total}] = best;
-  }
   return best;
-}
-
-template <int BN, int NB, int CS>
-void launch(const CUtensorMap& tmx, const CUtensorMap& tmw, const CUtensorMap& tmw2, const AwqDecParams& p, const AwqPlan& plan,
-            cudaStream_t st) {
-  configure_once<BN, NB, CS>();
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(static_cast<unsigned>(plan.tiles * CS));
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = AwqDecSmem<BN, NB>::bytes(plan.p_stages, CS);
-  cfg.stream = st;
-  cudaLaunchAttribute attr[2];
-  int na = 0;
-  if (CS > 1) {
-    attr[na].id = cudaLaunchAttributeClusterDimension;
-    attr[na].val.clusterDim.x = CS;
-    attr[na].val.clusterDim.y = 1;
-    attr[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  if (pdl_enabled()) {
-    attr[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[na].val.programmaticStreamSerializationAllowed = 1;
-    ++na;
-  }
-  cfg.attrs = attr;
-  cfg.numAttrs = na;
-  CT2_CUDA_CHECK(cudaLaunchKernelEx(&cfg, awq_decode_kernel<BN, NB, CS>, tmx, tmw, tmw2, p));
-  check_launch();
 }
 
 template <int BN, int NB>
 bool run(const void* x, const AwqNative& w, const AwqNative* w2, int64_t m, AwqDecParams p, cudaStream_t st) {
   const int sb_total = static_cast<int>(w.k / kSlotK);
-  const AwqPlan plan = plan_awq<BN, NB>(w.n, sb_total, sm_count_of_current_device());
+  const int sms = sm_count_of_current_device();
+  const Plan plan = cached_plan(w.n, sb_total, false,
+                                [&](int force_cs, int force_rows) { return plan_awq<BN, NB>(w.n, sb_total, sms, force_cs, force_rows); });
   if (plan.cs == 0) return false;
   p.d.n = w.n;
   p.d.m = m;
   p.d.kb_total = sb_total * kSub;
   p.sb_total = sb_total;
   p.d.tile_rows = plan.tile_rows;
-  p.d.stages = plan.p_stages;
-  p.k = w.k;
+  p.d.stages = plan.stages;
   p.group = w.group;
-  p.p_stages = plan.p_stages;
   p.sz[0] = static_cast<const __half2*>(w.sz);
   p.sz[1] = static_cast<const __half2*>(w2 ? w2->sz : w.sz);
   const CUtensorMap tmx = make_operand_map(x, m, w.k, 2, 1, BN);
   const CUtensorMap tmw = make_packed_map(w.wp, w.n, w.k, plan.tile_rows);
   const CUtensorMap tmw2 = make_packed_map(w2 ? w2->wp : w.wp, w.n, w.k, plan.tile_rows);
-  switch (plan.cs) {
-    case 1: launch<BN, NB, 1>(tmx, tmw, tmw2, p, plan, st); break;
-    case 2: launch<BN, NB, 2>(tmx, tmw, tmw2, p, plan, st); break;
-    case 3: launch<BN, NB, 3>(tmx, tmw, tmw2, p, plan, st); break;
-    default: launch<BN, NB, 4>(tmx, tmw, tmw2, p, plan, st); break;
-  }
+  dispatch_cs(plan.cs, [&](auto c) {
+    auto kernel = awq_decode_kernel<BN, NB, decltype(c)::value>;
+    allow_dynamic_smem(kernel, kMaxDynSmem);
+    launch_clustered(kernel, dim3(static_cast<unsigned>(plan.tiles * plan.cs)), dim3(kThreads), AwqDecSmem<BN, NB>::bytes(plan.stages, plan.cs),
+                     plan.cs, st, tmx, tmw, tmw2, p);
+  });
+  check_launch();
   return true;
 }
 

@@ -178,7 +178,7 @@ void launch_gemv(const void* x, const AwqNative& a, const AwqNative* b, const Ge
                                        static_cast<const __half*>(b->zr)} : w0;
   const int64_t groups = (a.n + R - 1) / R;        // row groups = warps at KS = 1
   const int force_ks = dec::env_int("CT2B200_AWQ_GEMV_KS", 0);
-  const bool split = force_ks ? force_ks == 2 : (groups < 2 * static_cast<int64_t>(dec::sm_count_of_current_device()) * kWarps && a.k >= 4096);
+  const bool split = force_ks ? force_ks == 2 : (groups < 2 * static_cast<int64_t>(sm_count_of_current_device()) * kWarps && a.k >= 4096);
   const dim3 block(kWarps * 32);
   if (split) {
     const dim3 grid(static_cast<unsigned>((groups * 2 + kWarps - 1) / kWarps));

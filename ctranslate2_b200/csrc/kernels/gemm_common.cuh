@@ -117,6 +117,22 @@ struct SplitKWorkspace {
   }
 };
 
+// SM count of the current device (cached per device)
+inline int sm_count_of_current_device() {
+  static std::mutex mu;
+  static std::map<int, int> cache;
+  int dev = 0;
+  cudaGetDevice(&dev);
+  std::lock_guard<std::mutex> lock(mu);
+  auto it = cache.find(dev);
+  if (it == cache.end()) {
+    int sms = 132;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    it = cache.emplace(dev, sms).first;
+  }
+  return it->second;
+}
+
 // Number of K splits: enough CTAs to cover every SM about twice, while each split keeps >= 4 K-tiles
 // and the partial planes fit the scratch.
 inline int choose_splits(int tiles, int k_tiles, int64_t accum_elems_needed, const SplitKWorkspace& w) {

@@ -71,13 +71,6 @@ struct PreParams {
   int64_t ldy;
 };
 
-template <int KIND> struct Elem { static constexpr int bytes = KIND == 0 ? 1 : 2; };
-
-__device__ __noinline__ float pre_act(float x, int act) {
-  if (act == CT2B200_ACT_SWISH) return __fdividef(x, 1.f + __expf(-x));
-  return apply_act(x, act);
-}
-
 __device__ __forceinline__ void epi_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 __device__ __forceinline__ void wg_sync(int half) { asm volatile("bar.sync %0, 128;" ::"r"(2 + half) : "memory"); }
 
@@ -243,7 +236,7 @@ __global__ void __launch_bounds__(kThreads, 1)
                   gate = __uint_as_float(r0[v0 + i]);
                   up = __uint_as_float(r1[v0 + i]);
                 }
-                gate = round_to<T>(pre_act(round_to<T>(gate), p.act));
+                gate = round_to<T>(act_call(round_to<T>(gate), p.act));
                 o.v[i] = from_f32<T>(gate * round_to<T>(up));
               }
               st16(yrow + c0 + v0, o);
@@ -262,7 +255,7 @@ __global__ void __launch_bounds__(kThreads, 1)
                 if constexpr (KIND == 0) v = __fdividef(static_cast<float>(static_cast<int32_t>(r0[v0 + i])), sa * ws[c]);
                 else v = __uint_as_float(r0[v0 + i]);
                 v = round_to<T>(round_to<T>(v) + bs[c]);
-                if (p.act >= 0) v = round_to<T>(pre_act(v, p.act));
+                if (p.act >= 0) v = round_to<T>(act_call(v, p.act));
                 if (rrow) v = v + to_f32(res[v0 / kVec].v[i]);
                 o.v[i] = from_f32<T>(v);
               }
@@ -299,14 +292,7 @@ void launch_prefill_bn(const void* x, const void* w, const void* w2, int64_t m, 
 template <typename T, int KIND, int NB>
 void launch_prefill(const void* x, const void* w, const void* w2, int64_t m, int64_t n, int64_t k, const PreParams& p,
                     cudaStream_t st) {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  static int cached_dev = -1, cached_sms = 132;
-  if (cached_dev != dev) {
-    cudaDeviceGetAttribute(&cached_sms, cudaDevAttrMultiProcessorCount, dev);
-    cached_dev = dev;
-  }
-  const int sms = cached_sms;
+  const int sms = sm_count_of_current_device();
   if constexpr (NB == 1) {
     // latency-bound regime: the wide tiles would run on fewer than a quarter of the SMs -> 64-column tiles (CT2B200_GEMM_PREFILL_BN pins)
     static const int force_bn = [] { const char* e = std::getenv("CT2B200_GEMM_PREFILL_BN"); return e ? std::atoi(e) : 0; }();

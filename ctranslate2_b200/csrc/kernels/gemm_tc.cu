@@ -29,11 +29,6 @@ namespace {
 
 using namespace tc;
 
-template <int KIND> struct KindTraits;
-template <> struct KindTraits<0> { using Acc = int32_t; static constexpr int kElem = 1; };
-template <> struct KindTraits<1> { using Acc = float; static constexpr int kElem = 2; };
-template <> struct KindTraits<2> { using Acc = float; static constexpr int kElem = 2; };
-
 struct TcParams {
   int64_t rows_a;      // rows of the M-side operand (n when swapped, m otherwise)
   int64_t rows_b;      // rows of the N-side operand
@@ -63,13 +58,6 @@ struct TcSmem {
   static constexpr int kStages = ((200 * 1024 - kAcc) / kStage) > 8 ? 8 : ((200 * 1024 - kAcc) / kStage);
   static constexpr size_t kBytes = kAcc + static_cast<size_t>(kStages) * kStage + 1024 /*align*/ + 256 /*barriers*/;
 };
-
-// Activation out of line: the epilogue is unrolled over the columns of a chunk, and inlining erff/tanhf/expf
-// into every unrolled copy made the kernels 20-30 k SASS instructions (0.3-0.5 MB), i.e. instruction-fetch bound.
-__device__ __noinline__ float apply_act_call(float x, int act) {
-  if (act == CT2B200_ACT_SWISH) return __fdividef(x, 1.f + __expf(-x));     // the hot one (SwiGLU)
-  return apply_act(x, act);
-}
 
 // Epilogue of one thread over kCols (16) consecutive N-side rows of its M-side row `arow`.
 //   kSwap: arow = output channel n, N-side rows = batch rows m;   !kSwap: arow = batch row m, N-side = channels n.
@@ -150,20 +138,20 @@ __device__ __forceinline__ void epi_finish(const TcParams& p, const uint32_t (&r
     if constexpr (KIND != 0) {
       v = round_to<T>(__uint_as_float(r[0][j]));
       if (has_bias) v = round_to<T>(v + in.bj[j]);
-      if (act >= 0) v = round_to<T>(apply_act_call(v, act));
+      if (act >= 0) v = round_to<T>(act_call(v, act));
       if (has_res) v = v + in.resj[j];
     } else if constexpr (NB == 2) {
       const float sx = kSwap ? in.sj0[j] : in.st0;
       const float sg = kSwap ? in.st0 : in.sj0[j], su = kSwap ? in.st1 : in.sj1[j];
       float gate = round_to<T>(__fdividef(static_cast<float>(static_cast<int32_t>(r[0][j])), sx * sg));
-      gate = round_to<T>(apply_act_call(gate, act));
+      gate = round_to<T>(act_call(gate, act));
       const float up = round_to<T>(__fdividef(static_cast<float>(static_cast<int32_t>(r[1][j])), sx * su));
       v = gate * up;
     } else {
       const float sx = kSwap ? in.sj0[j] : in.st0, sw = kSwap ? in.st0 : in.sj0[j];
       v = round_to<T>(__fdividef(static_cast<float>(static_cast<int32_t>(r[0][j])), sx * sw));
       if (has_bias) v = round_to<T>(v + in.bj[j]);
-      if (act >= 0) v = round_to<T>(apply_act_call(v, act));
+      if (act >= 0) v = round_to<T>(act_call(v, act));
       if (has_res) v = v + in.resj[j];
     }
     y[base + j * step] = from_f32<T>(v);
@@ -184,7 +172,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     gemm_tc_kernel(const __grid_constant__ CUtensorMap tm_x, const __grid_constant__ CUtensorMap tm_w,
                    const __grid_constant__ CUtensorMap tm_w2, const TcParams p) {
   using S = TcSmem<BN, NB, kSwap>;
-  constexpr int kElem = KindTraits<KIND>::kElem;
+  constexpr int kElem = Elem<KIND>::bytes;
   constexpr int BK = kSwizzleBytes / kElem;            // elements of K per stage
   constexpr int kStages = S::kStages;
   static_assert(BN * NB <= 128 && kStages >= 2, "the accumulators of a tile live in the registers of one warpgroup");
@@ -488,7 +476,7 @@ template <typename T, int KIND, int BN, int NB, bool kSwap>
 void launch_tc(const void* x, const void* w, const void* w2, int64_t m, int64_t n, int64_t k, TcParams p,
                cudaStream_t st) {
   using S = TcSmem<BN, NB, kSwap>;
-  constexpr int elem = KindTraits<KIND>::kElem;
+  constexpr int elem = Elem<KIND>::bytes;
   auto kernel = gemm_tc_kernel<T, KIND, BN, NB, kSwap>;
   allow_dynamic_smem(kernel, 226 * 1024);
   const CUtensorMap tmx = make_operand_map(x, m, k, elem, KIND, kSwap ? BN : kTileM);
@@ -552,21 +540,7 @@ void launch_tc(const void* x, const void* w, const void* w2, int64_t m, int64_t 
   p.fslots = reinterpret_cast<float*>(wsp.accum2);
   p.counters = wsp.counters;
   if (p.cluster_s >= 2) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(static_cast<unsigned>(ctas));
-    cfg.blockDim = dim3(kTcThreads);
-    cfg.dynamicSmemBytes = smem_bytes;
-    cfg.stream = st;
-    cudaLaunchAttribute attr[2];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = p.cluster_s;
-    attr[0].val.clusterDim.y = 1;
-    attr[0].val.clusterDim.z = 1;
-    attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[1].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 2 : 1;
-    CT2_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kernel, tmx, tmw, tmw2, p));
+    launch_clustered(kernel, dim3(static_cast<unsigned>(ctas)), dim3(kTcThreads), smem_bytes, p.cluster_s, st, tmx, tmw, tmw2, p);
     check_launch();
     return;
   }

@@ -62,29 +62,11 @@ void gemm_s8_glu_tc(const int8_t* A, const int8_t* Bgate, const int8_t* Bup, int
 void gemm_f16_tc(const void* A, const void* B, const void* bias, const void* residual, int act, int64_t M,
                  int64_t N, int64_t K, void* C, int dtype, cudaStream_t st);
 
-// Row pre-phase of the decode GEMM: the kernel quantizes its own activations (ops::Quantize or ops::RMSNorm + ops::Quantize
-// of x [M, K] in the GEMM's dtype, bit-identical to launch_quantize_rows / launch_rms_norm) into q / s before it stages them,
-// behind a grid barrier.  q must be the `A` pointer of the call and s the epilogue's a_scale; bar = 2 zero-initialised words.
-struct RowPre {
-  int mode = 0;                 // 1 Quantize, 2 RMSNorm + Quantize
-  const void* x = nullptr;      // [M, K] T
-  const void* gamma = nullptr;  // [K] T (mode 2)
-  float eps = 0.f;
-  unsigned* bar = nullptr;
-};
-// The Dense that follows in the decode step (same m): its int8 weights are prefetched into L2 while this one streams
-// (successor prefetch, gemm_decode_common.cuh).  w2 = the "up" matrix when the successor is a gate/up pair.
-struct NextWeights {
-  const void* w = nullptr;
-  const void* w2 = nullptr;
-  int64_t n = 0, k = 0;
-};
-// gemm_decode.cu (wgmma, m <= 64): false = shape (or pre-phase) not covered, use the general kernel (+ separate row kernel)
+// gemm_decode.cu (wgmma, m <= 64): false = shape not covered, use the general kernel
 bool gemm_s8_decode(const int8_t* A, const int8_t* B, int64_t M, int64_t N, int64_t K, const DenseEpilogue& epi,
-                    int dtype, cudaStream_t st, const RowPre* pre = nullptr, const NextWeights* next = nullptr);
+                    int dtype, cudaStream_t st);
 bool gemm_s8_glu_decode(const int8_t* A, const int8_t* Bgate, const int8_t* Bup, int64_t M, int64_t N, int64_t K,
-                        const GluEpilogue& glu, int dtype, cudaStream_t st, const RowPre* pre = nullptr,
-                        const NextWeights* next = nullptr);
+                        const GluEpilogue& glu, int dtype, cudaStream_t st);
 bool gemm_f16_decode(const void* A, const void* B, const void* bias, const void* residual, int act, int64_t M,
                      int64_t N, int64_t K, void* C, int dtype, cudaStream_t st);
 

@@ -1,6 +1,5 @@
-// row_ops.cuh — the "-> int8 row" producers of the decode step as ONE device function of 128 threads, shared by the
-// standalone row kernel (rowwise.cu, one CTA per row) and the row pre-phase of the weight-streaming GEMM (gemm_decode.cu),
-// so both produce bit-identical int8 rows and scales:
+// row_ops.cuh — the "-> int8 row" producers of the decode step as ONE device function of 128 threads, run by
+// the row kernel of rowwise.cu (one CTA per row):
 //   MODE 0: Quantize(x)                         ops::Quantize            src/ops/quantize_gpu.cu:57-105
 //   MODE 1: Quantize(T(RMSNorm(x, gamma)))      ops::RMSNorm + Quantize  src/ops/rms_norm_gpu.cu:19-63
 //   MODE 2: Quantize(T(a * b))                  ops::Mul + Quantize      src/layers/transformer.cc:31-37

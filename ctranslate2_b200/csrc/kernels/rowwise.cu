@@ -148,8 +148,7 @@ __global__ void __launch_bounds__(kRowThreads) mul_quantize_kernel(const T* __re
 
 // ---------------------------------------------------------------------------------------------
 // Register-resident fast path of the "-> int8 row" producers of the decode step (row_ops.cuh: MODE 0 Quantize, 1 RMSNorm +
-// Quantize, 2 Mul + Quantize, 3 RMSNorm written as T).  One CTA of 128 threads per row, one global round trip; the same
-// device function runs as the row pre-phase of the decode GEMM (gemm_decode.cu), bit-identically.
+// Quantize, 2 Mul + Quantize, 3 RMSNorm written as T).  One CTA of 128 threads per row, one global round trip.
 // ---------------------------------------------------------------------------------------------
 template <typename T, int MODE, int NV>
 __global__ void __launch_bounds__(rowop::kThreads) row_to_int8_kernel(const T* __restrict__ x, const T* __restrict__ aux,

@@ -21,6 +21,16 @@ constexpr int kSwizzleBytes = 128;       // bytes of K per smem row (= one 128B 
 constexpr uint64_t kEvictFirst = 0x12F0000000000000ull;
 constexpr uint64_t kEvictLast = 0x14F0000000000000ull;
 
+// operand kinds of the kernels: KIND = 0 s8 / 1 f16 / 2 bf16
+template <int KIND> struct Elem { static constexpr int bytes = KIND == 0 ? 1 : 2; };
+
+// Activation out of line: the epilogues are unrolled over the columns of a chunk, and inlining erff/tanhf/expf
+// into every unrolled copy made the kernels 20-30 k SASS instructions (0.3-0.5 MB), i.e. instruction-fetch bound.
+static __device__ __noinline__ float act_call(float x, int act) {
+  if (act == CT2B200_ACT_SWISH) return __fdividef(x, 1.f + __expf(-x));     // the hot one (SwiGLU)
+  return apply_act(x, act);
+}
+
 // ---- PTX wrappers ----
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
 

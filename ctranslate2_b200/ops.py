@@ -123,19 +123,8 @@ def dense_int8(xq, x_scale, w, w_scale, bias=None, residual=None, activation_typ
     return y
 
 
-_barrier_words = {}
-
-
-def _barrier(device):
-    """Grid-barrier words of the row pre-phase (two zero-initialised uint32), one buffer per device."""
-    key = str(device)
-    if key not in _barrier_words:
-        _barrier_words[key] = torch.zeros(64, dtype=torch.int32, device=device)
-    return _barrier_words[key]
-
-
 def dense_int8_rows(x, w, w_scale, gamma=None, eps=1e-5, bias=None, residual=None, activation_type=None):
-    """[RMSNorm +] Quantize + layers::Dense (INT8 arm) from rows in T: ONE launch for m <= 64.  Returns (y, xq, x_scale)."""
+    """[RMSNorm +] Quantize + layers::Dense (INT8 arm) from rows in T: the row kernel, then the fused Dense.  Returns (y, xq, x_scale)."""
     x, w = _c(x), _c(w)
     m, k = x.shape
     n = w.shape[0]
@@ -145,7 +134,7 @@ def dense_int8_rows(x, w, w_scale, gamma=None, eps=1e-5, bias=None, residual=Non
     act = -1 if activation_type is None else activation_type
     check(lib().ct2b200_dense_s8_rows(_p(x), _p(gamma), ctypes.c_float(eps), _p(w), _p(w_scale), _p(bias), _p(residual), act,
                                       ctypes.c_int64(m), ctypes.c_int64(n), ctypes.c_int64(k), _p(y), _dt(x), _p(xq), _p(xs),
-                                      _p(_barrier(x.device)), _stream()))
+                                      _stream()))
     return y, xq, xs
 
 
@@ -158,7 +147,7 @@ def dense_int8_glu_rows(x, w_gate, gate_scale, w_up, up_scale, gamma=None, eps=1
     xs = torch.empty((m,), dtype=torch.float32, device=x.device)
     check(lib().ct2b200_dense_s8_glu_rows(_p(x), _p(gamma), ctypes.c_float(eps), _p(_c(w_gate)), _p(gate_scale), _p(_c(w_up)),
                                           _p(up_scale), activation_type, ctypes.c_int64(m), ctypes.c_int64(n),
-                                          ctypes.c_int64(k), _p(h), _dt(x), _p(xq), _p(xs), _p(_barrier(x.device)), _stream()))
+                                          ctypes.c_int64(k), _p(h), _dt(x), _p(xq), _p(xs), _stream()))
     return h, xq, xs
 
 

@@ -96,16 +96,15 @@ CT2B200_API int ct2b200_dense_s8_glu(const int8_t* xq_d, const float* x_scale_d,
  * src/layers/common.cc:353-401 preceded by ops::Quantize (quantize.cc:21-50) or, with gamma_d, by the layer's pre-norm
  * ops::RMSNorm (rms_norm_gpu.cu:19-63):  xq, x_scale = Quantize([RMSNorm(x, gamma, eps)]);  y = dense_s8(xq, x_scale, ...).
  * x [m,k] T; xq_d [m,k] int8 and x_scale_d [m] are OUTPUTS (the same bits ct2b200_quantize_rows / ct2b200_rms_norm_quantize
- * produce).  Runs as the register-resident row kernel + the fused Dense under programmatic dependent launch; barrier_d is
- * unused. */
+ * produce).  Runs as the register-resident row kernel + the fused Dense under programmatic dependent launch. */
 CT2B200_API int ct2b200_dense_s8_rows(const void* x_d, const void* gamma_d, float eps, const int8_t* w_d, const float* w_scale_d,
                           const void* bias_d, const void* residual_d, int act, int64_t m, int64_t n, int64_t k,
-                          void* y_d, int dtype, int8_t* xq_d, float* x_scale_d, unsigned* barrier_d, void* stream);
+                          void* y_d, int dtype, int8_t* xq_d, float* x_scale_d, void* stream);
 /* same for the gate/up pair: h = act(dense(xq, w_gate)) * dense(xq, w_up) */
 CT2B200_API int ct2b200_dense_s8_glu_rows(const void* x_d, const void* gamma_d, float eps, const int8_t* w_gate_d,
                               const float* w_gate_scale_d, const int8_t* w_up_d, const float* w_up_scale_d, int act,
                               int64_t m, int64_t n, int64_t k, void* h_d, int dtype, int8_t* xq_d, float* x_scale_d,
-                              unsigned* barrier_d, void* stream);
+                              void* stream);
 
 /* primitives<Device::CUDA>::gemm<float16_t|bfloat16_t> (trans_b, alpha 1, beta 0) + ops::Gemm's
  * apply_bias_and_activation — src/cuda/primitives.cu:485-569, src/ops/gemm.cc:10-25.
