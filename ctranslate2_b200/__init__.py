@@ -4,7 +4,7 @@ There is no CPU or PyTorch fallback: importing works anywhere, every compute cal
 H100."""
 from . import ops  # noqa: F401
 from ._lib import Ct2B200Error, kernel_launch_count, lib  # noqa: F401
-from .generator import GenerationResult, Generator, model_summary  # noqa: F401
+from .generator import GenerationResult, Generator, ScoringResult, model_summary  # noqa: F401
 from .translator import TranslationResult, Translator, translator_summary  # noqa: F401
 from .whisper import Whisper, WhisperGenerationResult  # noqa: F401
 

@@ -198,6 +198,15 @@ CT2B200_API int ct2b200_softmax(const void* x, const int32_t* lengths, int64_t r
   });
 }
 
+CT2B200_API int ct2b200_log_softmax_gather(const void* x, const int32_t* ids, int64_t rows, int64_t cols, float* y, int dtype,
+                               void* stream) {
+  return guarded([&] {
+    require_device();
+    CT2_REQUIRE(cols >= 1, "log_softmax_gather: empty rows");
+    launch_log_softmax_gather(x, ids, rows, cols, y, dtype, S(stream));
+  });
+}
+
 CT2B200_API int ct2b200_topk(const void* x, int64_t rows, int64_t cols, int k, void* values, int32_t* indices, int dtype,
                  void* stream) {
   return guarded([&] {
@@ -417,6 +426,14 @@ CT2B200_API int ct2b200_forward_batch(ct2b200_generator* g, const int32_t* ids, 
   return guarded([&] {
     CT2_REQUIRE(g && ids && logits, "forward_batch: null argument");
     g->impl->forward(ids, batch, time, return_log_probs != 0, logits);
+  });
+}
+
+CT2B200_API int ct2b200_score_batch(ct2b200_generator* g, const int32_t* ids, const int32_t* lens, int64_t batch,
+                        int64_t max_len, int64_t offset, float* out_scores) {
+  return guarded([&] {
+    CT2_REQUIRE(g && ids && lens && out_scores, "score_batch: null argument");
+    g->impl->score(ids, lens, batch, max_len, offset, out_scores);
   });
 }
 

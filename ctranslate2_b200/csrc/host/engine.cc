@@ -989,6 +989,15 @@ void LlamaDecoder::project_rows(const int32_t* rows_d, int64_t n, void* logits_o
   project(gathered_.ptr, n, logits_out_d);
 }
 
+void LlamaDecoder::gather_hidden(const int32_t* rows_d, int64_t n, void* out_d) {
+  launch_gather_rows(x_.ptr, rows_d, n, mc_.d_model * dtype_size(dtype_), out_d, stream_);
+}
+
+void LlamaDecoder::project_hidden(const void* x_rows_d, int64_t rows, void* logits_out_d) {
+  CT2_REQUIRE(rows <= chunk_rows_, "project_hidden: too many rows for the activation arena");
+  project(x_rows_d, rows, logits_out_d);
+}
+
 void LlamaDecoder::reorder_cache(const int32_t* parent_d, int beam, int64_t rows, int64_t positions) {
   CT2_REQUIRE(tp_.world == 1, "beam search does not run tensor parallel");
   CT2_REQUIRE(rows <= max_batch_ && positions <= max_len_, "reorder_cache: exceeds the KV arena");
@@ -1057,10 +1066,12 @@ Generator::Generator(const std::string& model_dir, const ct2b200_generator_confi
 Generator::~Generator() {
   if (graph_) cudaGraphExecDestroy(graph_);
   if (host_pinned_) cudaFreeHost(host_pinned_);
+  if (score_pinned_) cudaFreeHost(score_pinned_);
 }
 
 // prefill `time` tokens per row from position 0, in row chunks that fit the activation arena
-void Generator::run_prefill(const int32_t* ids_d, int64_t batch, int64_t time) {
+void Generator::run_prefill(const int32_t* ids_d, int64_t batch, int64_t time,
+                            const std::function<void(int64_t, int64_t)>& after_chunk) {
   LlamaDecoder& d = *decoder_;
   const int64_t tc_max = std::max<int64_t>(1, d.prefill_chunk_rows() / batch);
   for (int64_t t0 = 0; t0 < time; t0 += tc_max) {
@@ -1069,6 +1080,7 @@ void Generator::run_prefill(const int32_t* ids_d, int64_t batch, int64_t time) {
     CT2_CUDA_CHECK(cudaMemcpy2DAsync(ids_d_.ptr, tc * sizeof(int32_t), ids_d + t0, time * sizeof(int32_t),
                                      tc * sizeof(int32_t), batch, cudaMemcpyDeviceToDevice, d.stream()));
     d.forward_prefill(ids_d_.as<int32_t>(), batch, tc, t0, nullptr, nullptr, 0);
+    if (after_chunk) after_chunk(t0, tc);
   }
 }
 
@@ -1340,6 +1352,81 @@ void Generator::forward(const int32_t* ids_h, int64_t batch, int64_t time, bool 
     CT2_CUDA_CHECK(cudaMemcpyAsync(logits_h + r0 * V, f32.ptr, n * V * sizeof(float), cudaMemcpyDeviceToHost, st));
     CT2_CUDA_CHECK(cudaStreamSynchronize(st));
   }
+}
+
+// Generator::score_batch (src/scoring.cc:6-66, language_model.cc:113-133): inputs = ids[:, :-1] go through the prompt pass
+// in time chunks.  After each chunk, and before the next one overwrites the hidden state, the rows of its scored positions
+// (offset <= t < len - 1: padding and positions before `offset` never reach the lm_head) are gathered into the slab; every
+// full slab goes through the final RMSNorm + lm_head (project(): INT8 / AWQ / float heads, the prefill GEMM above 64 rows)
+// and the fused LogSoftMax + Gather, which writes one float per position.  Only those floats come back to the host.
+void Generator::score(const int32_t* ids_h, const int32_t* lens_h, int64_t batch, int64_t max_len, int64_t offset,
+                      float* out_h) {
+  std::lock_guard<std::mutex> lock(mu_);
+  LlamaDecoder& d = *decoder_;
+  cudaStream_t st = d.stream();
+  CT2_REQUIRE(batch > 0 && batch <= d.max_batch(), "score_batch: batch size exceeds max_batch");
+  CT2_REQUIRE(max_len >= 1 && max_len - 1 <= d.max_length(), "score_batch: sequences exceed max_length of the KV arena");
+  CT2_REQUIRE(offset >= 0, "score_batch: offset must be >= 0");
+  const int64_t T = max_len - 1;                       // input positions per row
+  int64_t total = 0;
+  for (int64_t b = 0; b < batch; ++b) {
+    CT2_REQUIRE(lens_h[b] >= 0 && lens_h[b] <= max_len, "score_batch: a sequence length exceeds max_len");
+    total += std::max<int64_t>(0, lens_h[b] - 1 - offset);
+  }
+  std::fill(out_h, out_h + batch * T, 0.f);
+  if (total == 0) return;
+  const int64_t V = d.config().vocab, dm = d.config().d_model, es = dtype_size(d.dtype());
+  const int64_t cap = d.max_batch() * d.max_length();    // scored positions of the largest call
+  if (!score_slab_.ptr) {
+    // as many rows as 256 MB of logits hold, at least max_batch and at most one prompt-pass chunk
+    score_slab_rows_ = std::min(d.prefill_chunk_rows(), std::max(d.max_batch(), (static_cast<int64_t>(256) << 20) / (V * es)));
+    score_slab_.alloc(static_cast<size_t>(score_slab_rows_) * (V + dm) * es + 256);
+    score_idx_d_.alloc(static_cast<size_t>(2) * cap * sizeof(int32_t));
+    score_out_d_.alloc(static_cast<size_t>(cap) * sizeof(float));
+    CT2_CUDA_CHECK(cudaMallocHost(&score_pinned_, static_cast<size_t>(2) * cap * sizeof(int32_t)));
+  }
+  uint8_t* logits = score_slab_.as<uint8_t>();
+  uint8_t* hidden = logits + (static_cast<size_t>(score_slab_rows_) * V * es + 255) / 256 * 256;
+  int32_t* rows_d = score_idx_d_.as<int32_t>();         // per scored position: its row in the chunk's hidden state
+  int32_t* tgt_d = rows_d + cap;                        //                      and its target id
+  int32_t* rows_h = score_pinned_;
+  int32_t* tgt_h = score_pinned_ + cap;
+  std::vector<int64_t> dest(total);                     // its place in out_h
+  float* scores_d = score_out_d_.as<float>();
+
+  CT2_CUDA_CHECK(cudaMemcpy2DAsync(prompt_d_.ptr, T * sizeof(int32_t), ids_h, max_len * sizeof(int32_t), T * sizeof(int32_t),
+                                   batch, cudaMemcpyHostToDevice, st));
+  int64_t picked = 0, done = 0;                         // positions gathered into the slab / projected and scored
+  auto flush = [&](int64_t upto) {
+    const int64_t n = upto - done;
+    if (n == 0) return;
+    d.project_hidden(hidden, n, logits);
+    launch_log_softmax_gather(logits, tgt_d + done, n, V, scores_d + done, d.dtype(), st);
+    done = upto;
+  };
+  run_prefill(prompt_d_.as<int32_t>(), batch, T, [&](int64_t t0, int64_t tc) {
+    const int64_t first = picked;
+    for (int64_t b = 0; b < batch; ++b)
+      for (int64_t t = std::max(t0, offset); t < std::min<int64_t>(t0 + tc, lens_h[b] - 1); ++t) {
+        rows_h[picked] = static_cast<int32_t>(b * tc + (t - t0));
+        tgt_h[picked] = ids_h[b * max_len + t + 1];
+        dest[picked++] = b * T + (t - offset);
+      }
+    if (picked == first) return;
+    CT2_CUDA_CHECK(cudaMemcpyAsync(rows_d + first, rows_h + first, (picked - first) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    CT2_CUDA_CHECK(cudaMemcpyAsync(tgt_d + first, tgt_h + first, (picked - first) * sizeof(int32_t), cudaMemcpyHostToDevice, st));
+    for (int64_t p = first; p < picked;) {
+      const int64_t k = std::min(score_slab_rows_ - (p - done), picked - p);
+      d.gather_hidden(rows_d + p, k, hidden + (p - done) * dm * es);
+      p += k;
+      if (p - done == score_slab_rows_) flush(p);
+    }
+  });
+  flush(picked);
+  std::vector<float> vals(total);
+  CT2_CUDA_CHECK(cudaMemcpyAsync(vals.data(), scores_d, total * sizeof(float), cudaMemcpyDeviceToHost, st));
+  CT2_CUDA_CHECK(cudaStreamSynchronize(st));
+  for (int64_t i = 0; i < total; ++i) out_h[dest[i]] = vals[i];
 }
 
 void Generator::bench_decode(int64_t batch, int64_t prompt_len, int64_t steps, int64_t warmup, float* prefill_ms,

@@ -7,6 +7,7 @@
 #include <cuda_runtime.h>
 
 #include <cstdint>
+#include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -136,6 +137,11 @@ class LlamaDecoder {
 
   // project rows (indices into the rows of the last forward_prefill) of the hidden state to the vocabulary
   void project_rows(const int32_t* rows_d, int64_t n, void* logits_out_d);
+  // copy rows (indices into the rows of the last forward_prefill) of the hidden state to out_d [n, d_model] T
+  void gather_hidden(const int32_t* rows_d, int64_t n, void* out_d);
+  // final RMSNorm + lm_head of `rows` hidden rows x_rows_d [rows, d_model] T (at most prefill_chunk_rows()):
+  // logits_out_d [rows, vocab] T
+  void project_hidden(const void* x_rows_d, int64_t rows, void* logits_out_d);
   void* logits_buffer() const { return logits_.ptr; }       // [max_batch, vocab] T
   // Beam search on the contiguous per-row caches (Decoder::replicate_state / update_state, decoder.cc:33-139): the K/V rows are
   // re-gathered into a second cache set (allocated on first use) and the two sets swap roles.
@@ -230,12 +236,19 @@ class Generator {
   std::vector<TranslationHypotheses> generate_beam(const GenerationRequest& req);
   // Generator::forward_batch
   void forward(const int32_t* ids_h, int64_t batch, int64_t time, bool log_probs, float* logits_h);
+  // Generator::score_batch (src/scoring.cc:6-66): ids_h [batch, max_len] right-padded with valid ids, lens_h [batch] the
+  // sequence lengths.  out_h [batch, max_len - 1]: row b holds log P(ids[b][t + 1] | ids[b][..t]) for
+  // offset <= t < lens_h[b] - 1 at column t - offset, then zeros.
+  void score(const int32_t* ids_h, const int32_t* lens_h, int64_t batch, int64_t max_len, int64_t offset, float* out_h);
   void bench_decode(int64_t batch, int64_t prompt_len, int64_t steps, int64_t warmup, float* prefill_ms,
                     float* decode_ms, int64_t* launches);
   void bench_last_logits(int64_t batch, float* logits_h, int64_t logits_len);
 
  private:
-  void run_prefill(const int32_t* ids_d, int64_t batch, int64_t time);
+  // the prompt pass from position 0 in time chunks that fit the activation arena; after_chunk(t0, tc) runs once the hidden
+  // state of positions [t0, t0 + tc) is complete, before the next chunk overwrites it
+  void run_prefill(const int32_t* ids_d, int64_t batch, int64_t time,
+                   const std::function<void(int64_t t0, int64_t tc)>& after_chunk = nullptr);
   void build_step_graph(int64_t batch, int64_t min_length, int num_end_ids);
   void launch_step(int64_t batch, int64_t min_length, int num_end_ids);
 
@@ -250,6 +263,11 @@ class Generator {
   int32_t* host_pinned_ = nullptr;
   size_t host_pinned_elems_ = 0;
   std::unique_ptr<struct BeamSearchArena> beam_;   // created by the first beam search
+  // score_batch, allocated by the first call: lm_head slab (logits [slab_rows, vocab] T | hidden rows [slab_rows, d_model] T),
+  // per scored position its hidden-state row and target id (int32 [2, max_batch * max_length]), and its log-probability
+  DeviceBuffer score_slab_, score_idx_d_, score_out_d_;
+  int64_t score_slab_rows_ = 0;
+  int32_t* score_pinned_ = nullptr;        // host staging of the row / target ids (pinned: the copies stay asynchronous)
   cudaGraphExec_t graph_ = nullptr;
   int64_t graph_nodes_ = 0;
   int64_t graph_batch_ = -1, graph_min_len_ = -1;

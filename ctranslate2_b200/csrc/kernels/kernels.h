@@ -30,6 +30,9 @@ void launch_rotary(const void* x, const void* sin, const void* cos, int64_t batc
                    int64_t ndims, bool interleave, void* y, int dtype, cudaStream_t st);
 void launch_softmax(const void* x, const int32_t* lengths, int64_t rows, int64_t cols, bool log, void* y,
                     int dtype, cudaStream_t st);
+// LogSoftMax + Gather fused: y [rows] f32 = T(x[r, ids[r]] - logsumexp(x[r, :])) (NaN for an id outside [0, cols))
+void launch_log_softmax_gather(const void* x, const int32_t* ids, int64_t rows, int64_t cols, float* y, int dtype,
+                               cudaStream_t st);
 void launch_topk(const void* x, int64_t rows, int64_t cols, int k, void* values, int32_t* indices, int dtype,
                  cudaStream_t st);
 

@@ -283,6 +283,83 @@ __global__ void __launch_bounds__(kRowThreads) softmax_kernel(const T* __restric
 }
 
 // ---------------------------------------------------------------------------------------------
+// ops::LogSoftMax + ops::Gather(axis -1, batch_dims 1) fused (src/scoring.cc:50-56): y[row] = float(T(x[id] - max -
+// log(sum exp(x - max)))), the value softmax_kernel's log path stores at column id.  The row is read once: each thread keeps
+// a running (max, sum) over 16-byte vectors (scalar head up to the first aligned element, scalar tail), the pairs are merged
+// across the block, and the target element is read on its own.  The log-probabilities are never written back.  The exps of
+// one vector are summed in fp32, the running sums and the final difference in fp64: the result is then within one unit of
+// T's last place of the exact value also for fp32 rows of 128K columns, where an fp32 running sum is not.
+// ---------------------------------------------------------------------------------------------
+struct MaxSum { float m; double s; };
+__device__ __forceinline__ MaxSum max_sum_merge(MaxSum a, MaxSum b) {
+  const float m = fmaxf(a.m, b.m);
+  if (m == -INFINITY) return {m, 0.0};
+  return {m, a.s * expf(a.m - m) + b.s * expf(b.m - m)};
+}
+__device__ __forceinline__ MaxSum warp_max_sum(MaxSum v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1)
+    v = max_sum_merge(v, {__shfl_xor_sync(0xffffffffu, v.m, o), __shfl_xor_sync(0xffffffffu, v.s, o)});
+  return v;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kRowThreads) log_softmax_gather_kernel(const T* __restrict__ x,
+                                                                         const int32_t* __restrict__ ids, int64_t cols,
+                                                                         float* __restrict__ y) {
+  __shared__ MaxSum red[kRowThreads / 32];
+  constexpr int N = Vec16<T>::N;
+  const int64_t row = blockIdx.x;
+  const T* xr = x + row * cols;
+  // elements before the first 16-byte boundary (rows of an odd width start anywhere); T-aligned rows are assumed
+  const int64_t head = min(cols, static_cast<int64_t>(((16 - (reinterpret_cast<uintptr_t>(xr) & 15)) & 15) / sizeof(T)));
+  const int64_t nv = (cols - head) / N;
+  const T* xv = xr + head;
+  MaxSum acc{-INFINITY, 0.0};
+  auto add = [&](float v) {               // one scalar element
+    if (v > acc.m) {
+      acc.s = acc.s * expf(acc.m - v) + 1.0;
+      acc.m = v;
+    } else if (v != -INFINITY) {
+      acc.s += expf(v - acc.m);
+    }
+  };
+  if (threadIdx.x < head) add(to_f32(xr[threadIdx.x]));
+#pragma unroll 4
+  for (int64_t v = threadIdx.x; v < nv; v += blockDim.x) {
+    const Vec16<T> d = ld16(xv + v * N);
+    float f[N];
+    float vm = -INFINITY;
+#pragma unroll
+    for (int i = 0; i < N; ++i) {
+      f[i] = to_f32(d.v[i]);
+      vm = fmaxf(vm, f[i]);
+    }
+    const float m = fmaxf(acc.m, vm);
+    if (m == -INFINITY) continue;
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < N; ++i) s += expf(f[i] - m);
+    acc = {m, (m == acc.m ? acc.s : acc.s * expf(acc.m - m)) + s};
+  }
+  for (int64_t j = head + nv * N + threadIdx.x; j < cols; j += blockDim.x) add(to_f32(xr[j]));
+  acc = warp_max_sum(acc);
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) red[warp] = acc;
+  __syncthreads();
+  if (warp == 0) {
+    acc = lane < kRowThreads / 32 ? red[lane] : MaxSum{-INFINITY, 0.0};
+    acc = warp_max_sum(acc);
+    if (lane == 0) {
+      const int64_t id = ids[row];
+      // an id outside the row has no log-probability: NaN rather than a read past the row
+      const double v = static_cast<double>(to_f32(xr[id >= 0 && id < cols ? id : 0])) - acc.m - log(acc.s);
+      y[row] = id >= 0 && id < cols ? round_to<T>(static_cast<float>(v)) : NAN;
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------
 // ops::TopK (src/ops/topk_gpu.cu:181-335).  k passes of a block arg-max over (value desc, index asc):
 // a strict total order, so exact ties resolve lowest-index-first regardless of the reduction tree
 // (the reference's cub tree does not guarantee that — SURVEY §8 a17).  The input is not mutated:
@@ -430,6 +507,14 @@ void launch_softmax(const void* x, const int32_t* lengths, int64_t rows, int64_t
   if (rows == 0) return;
   CT2_DISPATCH_DTYPE(dtype, (softmax_kernel<T><<<rows, kRowThreads, 0, st>>>(static_cast<const T*>(x), lengths,
                                                                            cols, log, static_cast<T*>(y))));
+  check_launch();
+}
+
+void launch_log_softmax_gather(const void* x, const int32_t* ids, int64_t rows, int64_t cols, float* y, int dtype,
+                               cudaStream_t st) {
+  if (rows == 0) return;
+  CT2_DISPATCH_DTYPE(dtype, (log_softmax_gather_kernel<T><<<rows, kRowThreads, 0, st>>>(static_cast<const T*>(x), ids, cols,
+                                                                                       y)));
   check_launch();
 }
 

@@ -224,6 +224,21 @@ class LogSoftMax(SoftMax):
         super().__init__(True)
 
 
+def log_softmax_gather(logits, ids):
+    """ops::LogSoftMax then ops::Gather(axis=-1, batch_dims=1) as one launch (src/scoring.cc:50-56): logits [.., V] in T,
+    ids int [..] -> float32 [..] = float(T(log_softmax(logits)[.., ids])); the log-probabilities are not materialised."""
+    logits = _c(logits)
+    cols = logits.shape[-1]
+    rows = logits.numel() // cols if cols else 0
+    ids = _c(ids).to(torch.int32)
+    if ids.numel() != rows:
+        raise ValueError("log_softmax_gather: one id per row is required")
+    y = torch.empty(logits.shape[:-1], dtype=torch.float32, device=logits.device)
+    check(lib().ct2b200_log_softmax_gather(_p(logits), _p(ids), ctypes.c_int64(rows), ctypes.c_int64(cols), _p(y),
+                                           _dt(logits), _stream()))
+    return y
+
+
 class TopK:
     """ops::TopK(k)(x) -> (values, indices int32); ties: lowest index first."""
     def __init__(self, k: int, axis: int = -1):

@@ -142,6 +142,13 @@ CT2B200_API int ct2b200_rotary(const void* x_d, const void* sin_d, const void* c
 CT2B200_API int ct2b200_softmax(const void* x_d, const int32_t* lengths_d, int64_t rows, int64_t cols, int log, void* y_d,
                     int dtype, void* stream);
 
+/* ops::LogSoftMax followed by ops::Gather(axis=-1, batch_dims=1) — src/scoring.cc:50-56, src/ops/softmax_gpu.cu:190-256,
+ * src/ops/gather_gpu.cu — fused, without writing the log-probabilities: x_d [rows, cols] T (any width, any T-aligned
+ * address), ids_d int32 [rows]; y_d f32 [rows] = float(T(x[r, ids[r]] - max_r - log(sum exp(x[r, :] - max_r)))), NaN for an
+ * id outside [0, cols). */
+CT2B200_API int ct2b200_log_softmax_gather(const void* x_d, const int32_t* ids_d, int64_t rows, int64_t cols, float* y_d,
+                               int dtype, void* stream);
+
 /* ops::TopK::compute<Device::CUDA,T,int32_t> — include/ctranslate2/ops/topk.h, src/ops/topk_gpu.cu:181-335.
  * Descending values; exact ties resolve lowest index first (SURVEY §8 a17).  k <= 64. */
 CT2B200_API int ct2b200_topk(const void* x_d, int64_t rows, int64_t cols, int k, void* values_d, int32_t* indices_d,
@@ -286,6 +293,16 @@ CT2B200_API int ct2b200_generate_batch_beam(ct2b200_generator* g, const int32_t*
  * ids_h [batch, time] int32 host; logits_h [batch, time, vocab] f32 host. */
 CT2B200_API int ct2b200_forward_batch(ct2b200_generator* g, const int32_t* ids_h, int64_t batch, int64_t time,
                           int return_log_probs, float* logits_h);
+
+/* Generator::score_batch_async (src/generator.cc:27-40; models/language_model.cc:38-52, 113-133; src/scoring.cc:6-66) with
+ * ScoringOptions::offset: the log-probability of every token given its prefix, from one causal prompt pass over
+ * ids[:, :-1], LogSoftMax in the compute type, Gather of ids[:, 1:].
+ * ids_h [batch, max_len] int32 host, right-padded with valid ids; lens_h [batch] sequence lengths (<= max_len; a row
+ * shorter than 2 scores nothing); max_len - 1 <= max_length of the generator.  out_scores_h [batch, max_len - 1] f32 host:
+ * row b holds the scores of tokens offset + 1 .. lens_h[b] - 1, then zeros.  Truncation (Vocabulary::to_ids) and
+ * re-batching (src/batch_reader.cc) are the caller's. */
+CT2B200_API int ct2b200_score_batch(ct2b200_generator* g, const int32_t* ids_h, const int32_t* lens_h, int64_t batch,
+                        int64_t max_len, int64_t offset, float* out_scores_h);
 
 /* Split phases, device-timed, for bench.py: prefill `prompt_len-1` tokens then run `steps` decode
  * steps with inputs already resident in HBM.  Returns device milliseconds of each phase. */
