@@ -534,6 +534,14 @@ CT2B200_API int ct2b200_translator_info(const ct2b200_translator* t, int* encode
   });
 }
 
+CT2B200_API int ct2b200_translator_positions(const ct2b200_translator* t, int64_t* encoder, int64_t* decoder) {
+  return guarded([&] {
+    CT2_REQUIRE(t && encoder && decoder, "translator_positions: null argument");
+    *encoder = t->impl->encoder_positions();
+    *decoder = t->impl->decoder_positions();
+  });
+}
+
 CT2B200_API int ct2b200_translator_summary(const char* model_dir, char* json_out, size_t capacity) {
   return guarded([&] {
     CT2_REQUIRE(model_dir && json_out && capacity > 0, "translator_summary: null argument");
@@ -618,6 +626,15 @@ CT2B200_API int ct2b200_translator_encode(ct2b200_translator* t, const int32_t* 
   return guarded([&] {
     CT2_REQUIRE(t && source_ids && source_lens && memory, "translator_encode: null argument");
     t->impl->encode(source_ids, source_lens, batch, max_source_len, memory);
+  });
+}
+
+CT2B200_API int ct2b200_translator_score_batch(ct2b200_translator* t, const int32_t* source_ids, const int32_t* source_lens,
+                                   int64_t batch, int64_t max_source_len, const int32_t* target_ids, const int32_t* target_lens,
+                                   int64_t max_target_len, int64_t offset, float* out_scores) {
+  return guarded([&] {
+    CT2_REQUIRE(t && source_ids && source_lens && target_ids && target_lens && out_scores, "translator_score_batch: null argument");
+    t->impl->score(source_ids, source_lens, batch, max_source_len, target_ids, target_lens, max_target_len, offset, out_scores);
   });
 }
 

@@ -5,6 +5,7 @@
 // reordered by an index remap of the K/V arena, and the host only polls a "finished entries" counter.
 #pragma once
 
+#include <functional>
 #include <memory>
 #include <string>
 #include <vector>
@@ -93,6 +94,8 @@ class Translator {
   ~Translator();
   const Seq2SeqConfig& config() const { return mc_; }
   int dtype() const { return dtype_; }
+  int64_t encoder_positions() const { return enc_positions_; }
+  int64_t decoder_positions() const { return dec_positions_; }
 
   // Translator::translate_batch on token ids
   std::vector<TranslationHypotheses> translate(const TranslationRequest& req);
@@ -100,6 +103,12 @@ class Translator {
   void encode(const int32_t* ids_h, const int32_t* lens_h, int64_t batch, int64_t max_source_len, float* memory_h);
   // WhisperEncoder::operator(): features_h [batch, n_mels, frames] f32 -> memory_h [batch, frames / 2, d_model] f32
   void whisper_encode(const float* features_h, int64_t batch, int64_t frames, float* memory_h);
+  // Translator::score_batch on token ids (EncoderDecoderReplica::run_scoring, sequence_to_sequence.cc:235-261; scoring.cc:6-66):
+  // sources [batch, max_source_len] right-padded (lengths >= 1), targets [batch, max_target_len] = start token .. </s>
+  // right-padded; out_h [batch, max_target_len - 1] gets the log-probabilities of target tokens offset + 1 .. len - 1 of
+  // each row, then zeros.  One teacher-forced pass of the decoder per group of pairs; nothing of the search state changes.
+  void score(const int32_t* src_ids_h, const int32_t* src_lens_h, int64_t batch, int64_t max_source_len,
+             const int32_t* tgt_ids_h, const int32_t* tgt_lens_h, int64_t max_target_len, int64_t offset, float* out_h);
   // models::Whisper::generate; no_speech_h [batch] or null
   std::vector<TranslationHypotheses> whisper_generate(const WhisperRequest& req, float* no_speech_h);
   // device-timed phases for bench.py: encoder pass, then `steps` decoding steps of batch * beam rows
@@ -109,7 +118,9 @@ class Translator {
  private:
   void load_dense(const ModelFile& f, const std::string& prefix, DenseWeights& w);
   void load_norm(const ModelFile& f, const std::string& prefix, NormWeights& n);
+  void drop_graph();            // synchronises and destroys the captured step (its buffers are about to move)
   void ensure_arena(int64_t batch, int64_t src_len, int beam, int64_t max_steps);
+  void ensure_rows(int64_t entries, int64_t enc_rows, int64_t rows);
   // Dense on T rows (quantizes them for int8 weights); `pre` = the LayerNorm applied first (fused with the quantization)
   void dense(const DenseWeights& w, const NormWeights* pre, const void* x, int64_t rows, const void* residual, int act, void* y,
              bool prequantized = false, int64_t ldy = 0);
@@ -120,10 +131,13 @@ class Translator {
   void run_whisper_encoder(int64_t batch, int64_t frames);
   void run_search(const BeamState& bs, int64_t S, int64_t first_check);
   void project_memory(int64_t batch, int64_t S);
+  // the decoder layer stack on `rows` rows of x_; `self_attention(layer)` fills ctx_ from qkv_, and each run of
+  // `rows_per_entry` rows attends to one memory entry.  Returns whether xq_ / xs_ hold Quantize(x_).
+  bool run_decoder_layers(int64_t rows, int rows_per_entry, int64_t S, const std::function<void(int)>& self_attention);
   void decoder_step(int64_t rows, int beam, int64_t batch, int64_t S);
   void launch_or_capture_step(const BeamState& bs, int64_t S);
 
-  std::mutex mu_;                // translate / encode / bench are serialised per translator
+  std::mutex mu_;                // translate / score / encode / bench are serialised per translator
   Seq2SeqConfig mc_;
   int dtype_ = CT2B200_F32, device_ = 0, weight_type_ = CT2B200_WEIGHTS_STORED, sm_count_ = 132;
   bool use_graph_ = true;
@@ -138,7 +152,8 @@ class Translator {
   std::vector<DecoderLayerWeights> dec_;
 
   // arena (grown on demand)
-  int64_t cap_batch_ = 0, cap_src_ = 0, cap_rows_ = 0, cap_steps_ = 0;
+  int64_t cap_batch_ = 0, cap_src_ = 0, cap_steps_ = 0;          // search state
+  int64_t cap_entries_ = 0, cap_enc_rows_ = 0, cap_rows_ = 0;     // encoder entries / rows, activation rows
   int cap_beam_ = 0;
   DeviceBuffer src_ids_, src_lens_, x_, xn_, xq_, xs_, qkv_, ctx_, h_, q_, memory_;
   std::vector<DeviceBuffer> mem_kv_, self_k_, self_v_;
@@ -149,6 +164,9 @@ class Translator {
   int64_t cap_frames_ = 0;
   int32_t* host_pinned_ = nullptr;
   size_t host_pinned_elems_ = 0;
+  // score: logits slab [score_slab_rows_, vocab (padded)], per pass: decoder input ids | scored rows | their target ids, scores
+  DeviceBuffer score_logits_, score_ids_, score_out_;
+  int64_t score_slab_rows_ = 0;
 
   cudaGraphExec_t graph_ = nullptr;
   int64_t graph_nodes_ = 0;

@@ -30,9 +30,10 @@ void launch_rotary(const void* x, const void* sin, const void* cos, int64_t batc
                    int64_t ndims, bool interleave, void* y, int dtype, cudaStream_t st);
 void launch_softmax(const void* x, const int32_t* lengths, int64_t rows, int64_t cols, bool log, void* y,
                     int dtype, cudaStream_t st);
-// LogSoftMax + Gather fused: y [rows] f32 = T(x[r, ids[r]] - logsumexp(x[r, :])) (NaN for an id outside [0, cols))
+// LogSoftMax + Gather fused: y [rows] f32 = T(x[r, ids[r]] - logsumexp(x[r, :])) (NaN for an id outside [0, cols)); row r
+// starts at x + r * ld (ld = 0: cols)
 void launch_log_softmax_gather(const void* x, const int32_t* ids, int64_t rows, int64_t cols, float* y, int dtype,
-                               cudaStream_t st);
+                               cudaStream_t st, int64_t ld = 0);
 void launch_topk(const void* x, int64_t rows, int64_t cols, int k, void* values, int32_t* indices, int dtype,
                  cudaStream_t st);
 
@@ -175,6 +176,10 @@ void launch_attention_beam_self(const void* qkv, void* k_cache, void* v_cache, c
                                 int64_t rows, int max_len, int H, int D, float scale, void* out, int dtype, cudaStream_t st);
 void launch_attention_cross(const void* q, const void* kv, const int32_t* lengths, int64_t rows, int beam, int S, int H, int D,
                             float scale, void* out, int dtype, cudaStream_t st);
+// causal self-attention of `time` teacher-forced decoder positions per sequence: qkv [batch * time, 3d] (row b * time + t
+// attends to rows b * time + j, j <= t), out [batch * time, d]; no cache is written
+void launch_attention_causal(const void* qkv, int64_t batch, int time, int H, int D, float scale, void* out, int dtype,
+                             cudaStream_t st);
 // device state of BeamSearch::search (decoding.cc:425-720); N = batch * beam rows, `stride` = allocated steps per row
 struct BeamState {
   int batch = 0, beam = 1, vocab = 0, stride = 0, max_steps = 0, max_hyp = 0, max_candidates = 1, num_hypotheses = 1;

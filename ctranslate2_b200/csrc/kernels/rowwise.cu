@@ -306,11 +306,11 @@ __device__ __forceinline__ MaxSum warp_max_sum(MaxSum v) {
 template <typename T>
 __global__ void __launch_bounds__(kRowThreads) log_softmax_gather_kernel(const T* __restrict__ x,
                                                                          const int32_t* __restrict__ ids, int64_t cols,
-                                                                         float* __restrict__ y) {
+                                                                         int64_t ld, float* __restrict__ y) {
   __shared__ MaxSum red[kRowThreads / 32];
   constexpr int N = Vec16<T>::N;
   const int64_t row = blockIdx.x;
-  const T* xr = x + row * cols;
+  const T* xr = x + row * ld;
   // elements before the first 16-byte boundary (rows of an odd width start anywhere); T-aligned rows are assumed
   const int64_t head = min(cols, static_cast<int64_t>(((16 - (reinterpret_cast<uintptr_t>(xr) & 15)) & 15) / sizeof(T)));
   const int64_t nv = (cols - head) / N;
@@ -511,10 +511,10 @@ void launch_softmax(const void* x, const int32_t* lengths, int64_t rows, int64_t
 }
 
 void launch_log_softmax_gather(const void* x, const int32_t* ids, int64_t rows, int64_t cols, float* y, int dtype,
-                               cudaStream_t st) {
+                               cudaStream_t st, int64_t ld) {
   if (rows == 0) return;
   CT2_DISPATCH_DTYPE(dtype, (log_softmax_gather_kernel<T><<<rows, kRowThreads, 0, st>>>(static_cast<const T*>(x), ids, cols,
-                                                                                       y)));
+                                                                                       ld > 0 ? ld : cols, y)));
   check_launch();
 }
 

@@ -165,6 +165,9 @@ __global__ void __launch_bounds__(256) layer_norm_kernel(const T* __restrict__ x
 //         reordering beams never copies K/V (Decoder::update_state, decoder.cc:33-55, gathers the whole state instead)
 // MODE 2  cross-attention (attention.cc:371-440): q [N, d]; keys / values = column blocks of kv [B*S, 2d] of batch entry
 //         row / beam, j < lengths[row / beam] (the beams of an entry share the memory: replicate_state copies it instead)
+// MODE 3  decoder self-attention over T teacher-forced positions (the full-sequence decoder call of scoring, decoder.cc:13-26):
+//         q, k, v = column blocks of qkv [B*T, 3d]; keys of row (b, t) = rows (b, j), j <= t (the causal mask; positions past
+//         a sequence's length are computed and ignored, as in MODE 0); no cache is written
 // ---------------------------------------------------------------------------------------------
 struct AttnGeneric {
   const void* q;
@@ -180,7 +183,7 @@ struct AttnGeneric {
   void* k_cache;             // MODE 1: [N, max_len, d]
   void* v_cache;
   int64_t rows;              // query rows
-  int S;                     // keys per batch entry (MODE 0 / 2) or max_len (MODE 1)
+  int S;                     // keys per batch entry (MODE 0 / 2), max_len (MODE 1) or positions per sequence (MODE 3)
   int beam;
   int H, D;
   float scale;
@@ -209,7 +212,7 @@ __global__ void __launch_bounds__(kAttnWarps * 32) attention_generic_kernel(Attn
   for (int i = lane; i < D; i += 32) qs[i] = to_f32(qrow[i]);
 
   int nkeys;
-  int64_t base = 0;          // first key row (MODE 0 / 2)
+  int64_t base = 0;          // first key row (MODE 0 / 2 / 3)
   const int32_t* anc = nullptr;
   int step = 0;
   const T* kb = static_cast<const T*>(a.k);
@@ -217,6 +220,10 @@ __global__ void __launch_bounds__(kAttnWarps * 32) attention_generic_kernel(Attn
   if constexpr (MODE == 0) {
     const int64_t b = n / a.S;
     nkeys = a.lengths ? min(a.lengths[b], a.S) : a.S;
+    base = b * a.S;
+  } else if constexpr (MODE == 3) {
+    const int64_t b = n / a.S;
+    nkeys = static_cast<int>(n - b * a.S) + 1;
     base = b * a.S;
   } else if constexpr (MODE == 2) {
     const int64_t b = n / a.beam;
@@ -913,6 +920,29 @@ void launch_attention_encoder(const void* qkv, const int32_t* lengths, int64_t b
   a.scale = scale;
   a.max_keys = S;
   CT2_DISPATCH_DTYPE(dtype, (launch_attn_mode<T, 0>(a, st)));
+}
+
+void launch_attention_causal(const void* qkv, int64_t batch, int time, int H, int D, float scale, void* out, int dtype,
+                             cudaStream_t st) {
+  if (batch * time == 0) return;
+  const int64_t d = static_cast<int64_t>(H) * D;
+  const size_t es = dtype_size(dtype);
+  AttnGeneric a{};
+  a.q = qkv;
+  a.q_stride = 3 * d;
+  a.k = static_cast<const uint8_t*>(qkv) + d * es;
+  a.v = static_cast<const uint8_t*>(qkv) + 2 * d * es;
+  a.kv_stride = 3 * d;
+  a.out = out;
+  a.out_stride = d;
+  a.rows = batch * time;
+  a.S = time;
+  a.beam = 1;
+  a.H = H;
+  a.D = D;
+  a.scale = scale;
+  a.max_keys = time;
+  CT2_DISPATCH_DTYPE(dtype, (launch_attn_mode<T, 3>(a, st)));
 }
 
 void launch_attention_beam_self(const void* qkv, void* k_cache, void* v_cache, const int32_t* anc, const int32_t* step_ptr,

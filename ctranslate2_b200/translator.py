@@ -1,7 +1,7 @@
 """`ctranslate2.Translator` for Device::CUDA on H100, on top of the C-ABI engine (include/ct2b200.h, encoder-decoder path).
 
 Mirrors python/cpp/translator.cc / include/ctranslate2/translator.h: `translate_batch(source, ...)` with the
-TranslationOptions of include/ctranslate2/translation.h.  Token strings <-> ids (ctranslate2::Vocabulary: source /
+TranslationOptions of include/ctranslate2/translation.h, and `score_batch(source, target, ...)`.  Token strings <-> ids (ctranslate2::Vocabulary: source /
 target / shared vocabulary files, `add_source_bos` / `add_source_eos` / `decoder_start_token` of config.json) are handled
 here, as in models::SequenceToSequenceModel (src/models/sequence_to_sequence.cc:19-100); ids cross the boundary in HOST
 buffers.  The encoder, the decoder with cross-attention and the beam search run on the device."""
@@ -16,7 +16,7 @@ from typing import List, Optional, Sequence, Union
 import numpy as np
 
 from ._lib import GeneratorConfig, check, lib
-from .generator import _COMPUTE, _F16, _F32, _is_neutral  # noqa: F401
+from .generator import _COMPUTE, _F16, _F32, ScoringResult, _is_neutral, _non_negative_int, _rebatch, _truncate  # noqa: F401
 
 _FLOAT_OF_WEIGHTS = {"float16": 1, "bfloat16": 2}
 
@@ -68,6 +68,19 @@ def _load_vocabulary(model_path: str, name: str) -> Optional[List[str]]:
     return None
 
 
+def _index(x, side: str, row: int) -> int:
+    if isinstance(x, (bool, np.bool_)) or not isinstance(x, (int, np.integer)):
+        raise ValueError(f"score_batch: {side} {row} mixes token ids with {type(x).__name__} values")
+    return int(x)
+
+
+def _check_range(rows, vocab_size: int, side: str) -> None:
+    for b, row in enumerate(rows):
+        bad = [i for i in row if not 0 <= i < vocab_size]
+        if bad:
+            raise ValueError(f"score_batch: {side} id {bad[0]} of pair {b} is outside the vocabulary [0, {vocab_size})")
+
+
 class Translator:
     def __init__(self, model_path: str, device: str = "cuda", device_index: int = 0, compute_type: str = "default",
                  use_cuda_graph: bool = True, max_positions: int = 512):
@@ -100,6 +113,12 @@ class Translator:
         self._h = L.ct2b200_translator_open(model_path.encode(), ctypes.byref(cfg))
         if not self._h:
             raise RuntimeError(L.ct2b200_last_error().decode())
+        enc_pos, dec_pos = ctypes.c_int64(), ctypes.c_int64()
+        check(L.ct2b200_translator_positions(ctypes.c_void_p(self._h), ctypes.byref(enc_pos), ctypes.byref(dec_pos)))
+        self._encoder_positions, self._decoder_positions = enc_pos.value, dec_pos.value
+        # the model's embedding sizes: the reference appends <unk> to a vocabulary file that lacks it (src/vocabulary.cc:46-48)
+        info = self.info()
+        self._src_vocab_size, self._tgt_vocab_size = info["source_vocab"], info["target_vocab"]
 
     def __del__(self):
         self.close()
@@ -179,6 +198,87 @@ class Translator:
                 results[b] = TranslationResult([[self._target[i] for i in h] for h in hyp_ids], hyp_ids,
                                                [float(scores[j, h]) for h in range(len(hyp_ids))] if return_scores else [])
         return results
+
+    def score_batch(self, source, target, *, max_batch_size: int = 0, batch_type: str = "examples",
+                    max_input_length: int = 1024, offset: int = 0, asynchronous: bool = False) -> List[ScoringResult]:
+        """Translator.score_batch (python/cpp/translator.cc:504-531): the log-probability of every target token given the source
+        and the target prefix, one ScoringResult per (source, target) pair in request order.  Sources are token-string lists
+        (looked up with the model's special tokens, as translate_batch does) or id lists (taken as they are); targets are
+        token-string lists or id lists, and get the decoder start token (when the model has one) and </s> either way.  An
+        empty source is a token list: it gets the model's special tokens, as in the reference, and scores 0 for every
+        target token only when it is still empty.  Both
+        are truncated to max_input_length tokens, the target plus one for its start token, keeping </s> (Vocabulary::to_ids).
+        Results cover target tokens offset + 1 .. (ScoringOptions::offset) and end with "</s>".  Pairs are re-batched
+        longest source first by max_batch_size / batch_type; the scores do not depend on the batching."""
+        if asynchronous:
+            raise ValueError("score_batch: asynchronous=True is not supported (results are returned, not futures)")
+        max_batch_size = _non_negative_int("max_batch_size", max_batch_size)
+        max_input_length = _non_negative_int("max_input_length", max_input_length)
+        offset = _non_negative_int("offset", offset)
+        if batch_type not in ("examples", "tokens"):
+            raise ValueError(f"Invalid batch type: {batch_type}")
+        sources, targets = [list(r) for r in source], [list(r) for r in target]
+        if len(sources) != len(targets):
+            raise ValueError(f"score_batch: {len(sources)} sources but {len(targets)} targets")
+        if not sources:
+            return []
+        src_eos = self._src_to_id.get(self.eos_token, -1)
+        tgt_eos = self._tgt_to_id[self.eos_token]
+        start = self._config.get("decoder_start_token", "<s>")
+        start_ids = [] if start is None else [self._tgt_to_id[start]]
+        tgt_unk = self._tgt_to_id.get(self.unk_token, 0)
+        src_rows, tgt_rows = [], []
+        for b, (s, t) in enumerate(zip(sources, targets)):
+            s = self.source_ids(s) if (not s or isinstance(s[0], str)) else [_index(x, "source", b) for x in s]
+            src_rows.append(_truncate(s, max_input_length, src_eos))
+            if start is None and not t:
+                tgt_rows.append(None)                  # skip_scoring: nothing to score without a start token
+                continue
+            t = [self._tgt_to_id.get(x, tgt_unk) for x in t] if (t and isinstance(t[0], str)) else [_index(x, "target", b) for x in t]
+            tgt_rows.append(_truncate(start_ids + t + [tgt_eos], max_input_length + 1 if max_input_length else 0, tgt_eos))
+        _check_range(src_rows, self._src_vocab_size, "source")
+        _check_range([t for t in tgt_rows if t is not None], self._tgt_vocab_size, "target")
+        for b, s in enumerate(src_rows):
+            if len(s) > self._encoder_positions:
+                raise ValueError(f"score_batch: source {b} has {len(s)} tokens, more than the {self._encoder_positions} "
+                                 "positions of the encoder's position table (lower max_input_length)")
+        for b, t in enumerate(tgt_rows):
+            if t is not None and len(t) - 1 > self._decoder_positions:
+                raise ValueError(f"score_batch: target {b} needs {len(t) - 1} decoder positions, more than the "
+                                 f"{self._decoder_positions} of the model's position table (lower max_input_length)")
+        results = [ScoringResult([], []) for _ in sources]
+        run = []
+        for b, (s, t) in enumerate(zip(src_rows, tgt_rows)):
+            if t is None:
+                continue
+            if not s:                                  # skip_scoring: an empty source scores 0 for every target token
+                results[b] = ScoringResult([self._target_token(i) for i in t[1:]], [0.0] * (len(t) - 1))
+                continue
+            run.append(b)
+        p = ctypes.c_void_p
+        for idx in _rebatch([len(src_rows[b]) for b in run], max_batch_size, batch_type, len(run)):
+            idx = [run[i] for i in idx]
+            B = len(idx)
+            src_lens = np.array([len(src_rows[b]) for b in idx], np.int32)
+            tgt_lens = np.array([len(tgt_rows[b]) for b in idx], np.int32)
+            S, T = int(src_lens.max()), int(tgt_lens.max())
+            src = np.zeros((B, S), np.int32)
+            tgt = np.zeros((B, T), np.int32)
+            for j, b in enumerate(idx):
+                src[j, :src_lens[j]] = src_rows[b]
+                tgt[j, :tgt_lens[j]] = tgt_rows[b]
+            out = np.zeros((B, T - 1), np.float32)
+            check(lib().ct2b200_translator_score_batch(
+                p(self._h), src.ctypes.data_as(p), src_lens.ctypes.data_as(p), ctypes.c_int64(B), ctypes.c_int64(S),
+                tgt.ctypes.data_as(p), tgt_lens.ctypes.data_as(p), ctypes.c_int64(T), ctypes.c_int64(offset),
+                out.ctypes.data_as(p)))
+            for j, b in enumerate(idx):
+                n = max(0, int(tgt_lens[j]) - 1 - offset)
+                results[b] = ScoringResult([self._target_token(i) for i in tgt_rows[b][1 + offset:]], out[j, :n].tolist())
+        return results
+
+    def _target_token(self, i: int) -> str:
+        return self._target[i] if i < len(self._target) else self.unk_token
 
     def _end_ids(self, end_token) -> List[int]:
         if end_token is None:

@@ -340,6 +340,8 @@ CT2B200_API ct2b200_translator* ct2b200_translator_open(const char* model_dir, c
 CT2B200_API void ct2b200_translator_close(ct2b200_translator* t);
 CT2B200_API int ct2b200_translator_info(const ct2b200_translator* t, int* encoder_layers, int* decoder_layers, int* num_heads,
                             int* d_model, int* source_vocab, int* target_vocab, int64_t* weight_bytes);
+/* Positions the encoder / decoder position tables hold (stored tables, or the sinusoidal encodings reserved at open). */
+CT2B200_API int ct2b200_translator_positions(const ct2b200_translator* t, int64_t* encoder, int64_t* decoder);
 /* Host only: the geometry parse_seq2seq_config reads from `model_dir`, as JSON. */
 CT2B200_API int ct2b200_translator_summary(const char* model_dir, char* json_out, size_t capacity);
 
@@ -364,6 +366,20 @@ CT2B200_API int ct2b200_beam_decide_host(int beam_size, const int32_t* words_h, 
 /* TransformerEncoder::operator() — memory_h [batch, max_source_len, d_model] f32 host (padded positions are unspecified). */
 CT2B200_API int ct2b200_translator_encode(ct2b200_translator* t, const int32_t* source_ids_h, const int32_t* source_lens_h,
                               int64_t batch, int64_t max_source_len, float* memory_h);
+/* Translator::score_batch (python/cpp/translator.cc:504-531; EncoderDecoderReplica::run_scoring,
+ * src/models/sequence_to_sequence.cc:235-261; src/scoring.cc:6-66) with ScoringOptions::offset: the log-probability of every
+ * target token given the source and the target prefix, from one teacher-forced decoder pass over target_ids[:, :-1] with
+ * causal self-attention, LogSoftMax in the compute type, Gather of target_ids[:, 1:].
+ * source_ids_h [batch, max_source_len] int32 host, right-padded; source_lens_h [batch] in [1, max_source_len] (empty sources
+ * are the caller's: skip_scoring gives them zeros).  target_ids_h [batch, max_target_len] int32 host = decoder start token (if
+ * the model has one), target tokens, </s>, right-padded; target_lens_h [batch] in [0, max_target_len] (a row shorter than 2
+ * scores nothing); max_target_len - 1 <= the decoder's position table.  out_scores_h [batch, max_target_len - 1] f32 host: row b
+ * holds the scores of target tokens offset + 1 .. target_lens_h[b] - 1, then zeros.  Vocabulary lookup, truncation
+ * (Vocabulary::to_ids) and re-batching (src/batch_reader.cc) are the caller's; pairs are run in the given order, split into
+ * decoder passes of bounded size inside the call. */
+CT2B200_API int ct2b200_translator_score_batch(ct2b200_translator* t, const int32_t* source_ids_h, const int32_t* source_lens_h,
+                                   int64_t batch, int64_t max_source_len, const int32_t* target_ids_h,
+                                   const int32_t* target_lens_h, int64_t max_target_len, int64_t offset, float* out_scores_h);
 /* Device-timed phases for bench.py: one encoder pass of [batch, source_len], then `steps` beam-search steps of
  * batch * beam_size rows with inputs resident in HBM. */
 CT2B200_API int ct2b200_bench_translate(ct2b200_translator* t, int64_t batch, int64_t source_len, int beam_size, int64_t steps,

@@ -276,6 +276,64 @@ def make_seq2seq_fixture():
     print("seq2seq fixture:", sum(len(m["cases"]) for e in fixture.values() for m in e["models"].values()), "cases")
 
 
+def _ref_translate_score(model_dir, compute, pairs, max_input_length, offset):
+    """Translator::score_batch of the unmodified reference (CPU) through tools/ref_translate_score.cc, built by
+    tools/ref_translate_score.mk against oracle/_ref/libct2ref.so into a temporary directory: one (tokens, log_probs) per
+    (source tokens, target tokens) pair."""
+    import subprocess
+    import tempfile
+    out_dir = os.path.join(tempfile.gettempdir(), "ct2ref_score")
+    subprocess.run(["make", "-s", "-f", "tools/ref_translate_score.mk", "score", "SCORE_OUT=" + out_dir], cwd=ROOT, check=True)
+    exe = os.path.join(out_dir, "ref_translate_score")
+    text = "%s\t%s\t%d\t%d\t0\n" % (model_dir, compute, max_input_length, offset)
+    text += "".join(" ".join(s) + "\t" + " ".join(t) + "\n" for s, t in pairs)
+    out = subprocess.run([exe], input=text.encode(), capture_output=True, check=True).stdout.decode()
+    res = []
+    for line in out.split("\n")[:len(pairs)]:
+        toks, scores = line.split("\t")
+        res.append((toks.split(" ") if toks else [], [float(x) for x in scores.split(" ")] if scores else []))
+    assert len(res) == len(pairs)
+    return res
+
+
+def make_translator_score_fixture():
+    """Translator::score_batch of the UNMODIFIED reference (oracle/_ref, CPU) on token strings: aren-transliteration in float32,
+    aren-transliteration-i8 in int8, and the post-norm / Swish / zero-first-embedding model in float32 and int8.  Ragged
+    batches, offsets 0 / 1 / 3, a max_input_length that truncates both sides, an empty source, unknown target tokens (the
+    post-norm model's vocabularies hold <unk>; the aren ones do not, and the reference maps unknown tokens past the output
+    layer there)."""
+    from ctranslate2_b200.translator import _load_vocabulary
+    models = [("aren-float32", "aren-transliteration", "float32"), ("aren-int8", "aren-transliteration-i8", "int8"),
+              ("postnorm-float32", "tiny_seq2seq_postnorm", "float32"), ("postnorm-int8", "tiny_seq2seq_postnorm", "int8")]
+    fixture = {"models": {}}
+    for name, mdir, compute in models:
+        path = os.path.join(OUT, mdir)
+        svocab = _load_vocabulary(path, "source_vocabulary")[3:]
+        tvocab = _load_vocabulary(path, "target_vocabulary")[3:]
+        svocab = [t for t in svocab if t not in ("<unk>", "<s>", "</s>", "<blank>")]
+        tvocab = [t for t in tvocab if t not in ("<unk>", "<s>", "</s>", "<blank>")]
+        rng = np.random.default_rng(21)
+        pick = lambda vocab, n: [vocab[int(i)] for i in rng.integers(0, len(vocab), size=n)]   # noqa: E731
+        ragged = [(pick(svocab, int(a)), pick(tvocab, int(b))) for a, b in zip(rng.integers(1, 14, size=7),
+                                                                               rng.integers(0, 14, size=7))]
+        edge = [([], pick(tvocab, 4)), (pick(svocab, 5), pick(tvocab, 6)), (pick(svocab, 2), [])]
+        if name.startswith("aren"):
+            # the pairs the reference's own Python test scores (python/tests/test_translator.py, test_score_api)
+            edge.append((["\u0622", "\u062a", "\u0632", "\u0645", "\u0648", "\u0646"], ["a", "t", "z", "m", "o", "n"]))
+        else:
+            edge.append((pick(svocab, 6), pick(tvocab, 2) + ["not-a-token"] + pick(tvocab, 3) + ["also-unknown"]))
+        cases = []
+        for pairs, max_len, offset in ((ragged, 1024, 0), (ragged, 1024, 1), (ragged, 1024, 3), (ragged, 5, 0),
+                                       (ragged, 5, 1), (edge, 1024, 0), (edge, 1024, 2)):
+            res = _ref_translate_score(path, compute, pairs, max_len, offset)
+            cases.append({"source": [p[0] for p in pairs], "target": [p[1] for p in pairs], "max_input_length": max_len,
+                          "offset": offset, "tokens": [r[0] for r in res], "log_probs": [r[1] for r in res]})
+        fixture["models"][name] = {"model": mdir, "compute_type": compute, "cases": cases}
+    with open(os.path.join(OUT, "seq2seq_score_ref.json"), "w") as f:
+        json.dump(fixture, f, ensure_ascii=False)
+    print("translator score fixture:", sum(len(m["cases"]) for m in fixture["models"].values()), "cases")
+
+
 WHISPER_CASES = [  # (beam, num_hypotheses, length_penalty, max_length, suppress_blank, timestamps)
     (1, 1, 1.0, 24, True, False), (3, 2, 1.0, 24, True, False), (5, 3, 1.0, 30, True, False), (5, 1, 0.0, 24, False, False),
     (2, 2, 0.7, 16, True, False), (1, 1, 1.0, 30, True, True), (5, 2, 1.0, 30, True, True), (3, 3, 1.0, 24, False, True)]
@@ -339,6 +397,9 @@ def main():
         return
     if "--seq2seq-only" in sys.argv:
         make_seq2seq_fixture()
+        return
+    if "--translator-score-only" in sys.argv:
+        make_translator_score_fixture()
         return
     if "--processors-only" in sys.argv:
         make_processors_fixture()
@@ -411,6 +472,7 @@ def main():
     make_ragged_fixture()
     make_score_fixture()
     make_seq2seq_fixture()
+    make_translator_score_fixture()
     make_whisper_fixture()
     print("done")
 
