@@ -6,6 +6,6 @@ from . import ops  # noqa: F401
 from ._lib import Ct2B200Error, kernel_launch_count, lib  # noqa: F401
 from .generator import GenerationResult, Generator, ScoringResult, model_summary  # noqa: F401
 from .translator import TranslationResult, Translator, translator_summary  # noqa: F401
-from .whisper import Whisper, WhisperGenerationResult  # noqa: F401
+from .whisper import Whisper, WhisperAlignmentResult, WhisperGenerationResult  # noqa: F401
 
 __version__ = "0.1.0"

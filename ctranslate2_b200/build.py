@@ -17,7 +17,7 @@ OUT = os.path.join(HERE, "libct2b200.so")
 OBJ = os.path.join(HERE, "_build")
 SOURCES = [
     "kernels/rowwise.cu", "kernels/tp_rows.cu", "kernels/gemm_s8_mma.cu", "kernels/gemm_tc.cu", "kernels/gemm_decode.cu", "kernels/gemm_prefill.cu", "kernels/awq.cu", "kernels/awq_decode.cu", "kernels/awq_gemv.cu", "kernels/attention.cu", "kernels/attention_mma.cu", "kernels/attention_decode.cu",
-    "kernels/decode_loop.cu", "kernels/seq2seq.cu", "host/engine.cc", "host/beam.cc", "host/translator.cc", "c_api.cc",
+    "kernels/decode_loop.cu", "kernels/seq2seq.cu", "kernels/whisper_align.cu", "host/engine.cc", "host/beam.cc", "host/translator.cc", "c_api.cc",
 ]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-std=c++17", "-O3", "-lineinfo", "-Xcompiler", "-fPIC",

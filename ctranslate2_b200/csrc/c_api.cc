@@ -8,6 +8,7 @@
 
 #include "common.cuh"
 #include "host/beam.h"
+#include "host/dtw.h"
 #include "host/engine.h"
 #include "host/translator.h"
 #include "kernels/beam_decide.h"
@@ -702,6 +703,65 @@ CT2B200_API int ct2b200_whisper_generate(ct2b200_translator* t, const float* fea
         out_lens[b * num_hypotheses + h] = have ? static_cast<int32_t>(len) : -1;
         out_scores[b * num_hypotheses + h] = have ? res[b].scores[h] : 0.f;
       }
+  });
+}
+
+CT2B200_API int ct2b200_whisper_align(ct2b200_translator* t, const float* features, int64_t batch, int64_t frames,
+                                      const int32_t* start_ids, int64_t start_len, const int32_t* text_ids, const int32_t* text_lens,
+                                      int64_t max_text, const int32_t* num_frames, int median_filter_width, const int32_t* heads,
+                                      int num_heads, int32_t no_timestamps_id, int32_t eot_id, int32_t* out_path,
+                                      int32_t* out_path_lens, float* out_probs, float* matrix) {
+  return guarded([&] {
+    CT2_REQUIRE(t && features && start_ids && text_lens && num_frames && heads && out_path && out_path_lens && out_probs,
+                "whisper_align: null argument");
+    CT2_REQUIRE(max_text == 0 || text_ids, "whisper_align: null argument");
+    WhisperAlignRequest r;
+    r.features = features;
+    r.batch = batch;
+    r.frames = frames;
+    r.start = start_ids;
+    r.start_len = start_len;
+    r.text = text_ids;
+    r.text_lens = text_lens;
+    r.max_text = max_text;
+    r.num_frames = num_frames;
+    r.median_filter_width = median_filter_width;
+    for (int i = 0; i < num_heads; ++i) r.heads.emplace_back(heads[2 * i], heads[2 * i + 1]);
+    r.no_timestamps_id = no_timestamps_id;
+    r.eot_id = eot_id;
+    const std::vector<WhisperAlignResult> res = t->impl->whisper_align(r, matrix);
+    const int64_t max_path = max_text + 1 + (frames + 1) / 2;
+    for (int64_t b = 0; b < batch; ++b) {
+      const auto& p = res[b].path;
+      CT2_REQUIRE(static_cast<int64_t>(p.size()) <= max_path, "whisper_align: path longer than expected");
+      for (size_t i = 0; i < p.size(); ++i) {
+        out_path[(b * max_path + i) * 2] = static_cast<int32_t>(p[i].first);
+        out_path[(b * max_path + i) * 2 + 1] = static_cast<int32_t>(p[i].second);
+      }
+      out_path_lens[b] = static_cast<int32_t>(p.size());
+      for (int64_t i = 0; i < max_text; ++i)
+        out_probs[b * max_text + i] = i < static_cast<int64_t>(res[b].text_token_probs.size()) ? res[b].text_token_probs[i] : 0.f;
+    }
+  });
+}
+
+CT2B200_API int ct2b200_whisper_detect_language(ct2b200_translator* t, const float* features, int64_t batch, int64_t frames,
+                                                int32_t sot_id, const int32_t* lang_ids, int num_langs, float* probs) {
+  return guarded([&] {
+    CT2_REQUIRE(t && features && lang_ids && probs, "whisper_detect_language: null argument");
+    t->impl->whisper_detect_language(features, batch, frames, sot_id, std::vector<int32_t>(lang_ids, lang_ids + num_langs), probs);
+  });
+}
+
+CT2B200_API int ct2b200_negative_dtw_host(const float* x, int64_t n, int64_t m, int32_t* out_path, int32_t* out_len) {
+  return guarded([&] {
+    CT2_REQUIRE(x && out_path && out_len && n >= 1 && m >= 1, "negative_dtw_host: bad argument");
+    const auto p = negative_dtw(x, n, m);
+    for (size_t i = 0; i < p.size(); ++i) {
+      out_path[2 * i] = static_cast<int32_t>(p[i].first);
+      out_path[2 * i + 1] = static_cast<int32_t>(p[i].second);
+    }
+    *out_len = static_cast<int32_t>(p.size());
   });
 }
 

@@ -5,6 +5,8 @@
 
 #include <cuda_profiler_api.h>
 
+#include "dtw.h"
+
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
@@ -314,12 +316,7 @@ void Translator::ensure_arena(int64_t batch, int64_t src_len, int beam, int64_t 
       self_v_[l].alloc(N * L * d * es);
     }
     logits_.alloc(N * ((V + 7) / 8 * 8) * es);
-    if (mc_.whisper) {
-      const int64_t frames = 2 * S;                        // conv2 halves the frames
-      features_.alloc(B * mc_.n_mels * frames * 4);
-      cols_.alloc(std::max(B * frames * mc_.n_mels * 3, B * S * d * 3) * es);
-      conv_out_.alloc(B * frames * d * es);
-    }
+    if (mc_.whisper) ensure_whisper_frontend(B, S);
     const size_t need = static_cast<size_t>(B) * S + B + 64 + static_cast<size_t>(N) * 16 + 8192;
     if (need > host_pinned_elems_) {
       if (host_pinned_) cudaFreeHost(host_pinned_);
@@ -328,6 +325,17 @@ void Translator::ensure_arena(int64_t batch, int64_t src_len, int beam, int64_t 
     }
   }
   ensure_rows(cap_batch_, cap_batch_ * cap_src_, std::max(cap_batch_ * cap_src_, cap_batch_ * cap_beam_));
+}
+
+void Translator::ensure_whisper_frontend(int64_t batch, int64_t S) {
+  if (batch <= cap_fe_batch_ && S <= cap_fe_src_) return;
+  cap_fe_batch_ = std::max(cap_fe_batch_, batch);
+  cap_fe_src_ = std::max(cap_fe_src_, S);
+  const size_t es = dtype_size(dtype_);
+  const int64_t B = cap_fe_batch_, frames = 2 * cap_fe_src_, d = mc_.d_model;   // conv2 halves the frames
+  features_.alloc(B * mc_.n_mels * frames * 4);
+  cols_.alloc(std::max(B * frames * mc_.n_mels * 3, B * cap_fe_src_ * d * 3) * es);
+  conv_out_.alloc(B * frames * d * es);
 }
 
 // Encoder entries (source lengths), encoder rows (source ids, memory, memory keys / values: entries x padded source length)
@@ -441,7 +449,8 @@ void Translator::project_memory(int64_t batch, int64_t S) {
 
 // TransformerDecoder::decode's layer loop (transformer.cc:621-871), shared by the one-token step and the teacher-forced pass:
 // only the self-attention differs.  Cross-attention: row n reads memory entry n / rows_per_entry.
-bool Translator::run_decoder_layers(int64_t rows, int rows_per_entry, int64_t S, const std::function<void(int)>& self_attention) {
+bool Translator::run_decoder_layers(int64_t rows, int rows_per_entry, int64_t S, const std::function<void(int)>& self_attention,
+                                    const std::vector<AttnCapture>* capture) {
   const float scale = 1.f / std::sqrt(static_cast<float>(mc_.head_dim));
   const bool pre = mc_.dec_pre_norm;
   bool xq = false;                                 // xq_ / xs_ already hold Quantize(x_) (left by a post-norm launch)
@@ -452,8 +461,12 @@ bool Translator::run_decoder_layers(int64_t rows, int rows_per_entry, int64_t S,
     dense(w.self.out, nullptr, ctx_.ptr, rows, x_.ptr, -1, x_.ptr);
     xq = !pre && post_norm(w.self.norm, x_.ptr, rows, &w.cross.in);
     dense(w.cross.in, pre ? &w.cross.norm : nullptr, x_.ptr, rows, nullptr, -1, q_.ptr, xq);
-    launch_attention_cross(q_.ptr, mem_kv_[l].ptr, src_lens_.as<int32_t>(), rows, rows_per_entry, static_cast<int>(S),
-                           mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, dtype_, stream_);
+    if (capture && (*capture)[l].masks)
+      launch_attention_cross_capture(q_.ptr, mem_kv_[l].ptr, src_lens_.as<int32_t>(), rows, rows_per_entry, static_cast<int>(S),
+                                     mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, (*capture)[l], dtype_, stream_);
+    else
+      launch_attention_cross(q_.ptr, mem_kv_[l].ptr, src_lens_.as<int32_t>(), rows, rows_per_entry, static_cast<int>(S),
+                             mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, dtype_, stream_);
     dense(w.cross.out, nullptr, ctx_.ptr, rows, x_.ptr, -1, x_.ptr);
     xq = !pre && post_norm(w.cross.norm, x_.ptr, rows, &w.ffn.ff1);
     dense(w.ffn.ff1, pre ? &w.ffn.norm : nullptr, x_.ptr, rows, nullptr, mc_.dec_activation, h_.ptr, xq);
@@ -625,12 +638,7 @@ void Translator::score(const int32_t* src_ids_h, const int32_t* src_lens_h, int6
   std::fill(out_h, out_h + batch * Tout, 0.f);
   const int64_t V = mc_.tgt_vocab, d = mc_.d_model;
   const size_t es = dtype_size(dtype_);
-  // row stride of the logits: the INT8 epilogue stores 16-byte rows (set_logits_ld)
-  const int64_t ld = projection_.kind == DenseWeights::INT8 ? (V + 7) / 8 * 8 : V;
-  if (!score_logits_.ptr) {
-    score_slab_rows_ = std::max<int64_t>(1, std::min<int64_t>(kScoreSlabRows, (static_cast<int64_t>(256) << 20) / (ld * es)));
-    score_logits_.alloc(static_cast<size_t>(score_slab_rows_) * ld * es);
-  }
+  const int64_t ld = ensure_score_slab();
   const float scale = 1.f / std::sqrt(static_cast<float>(mc_.head_dim));
   for (int64_t p0 = 0; p0 < batch;) {
     // pairs p0 .. p1 - 1, padded to Sp source and Tp decoder positions
@@ -690,6 +698,18 @@ void Translator::score(const int32_t* src_ids_h, const int32_t* src_lens_h, int6
     CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));     // also keeps the staging vectors alive until their copies are done
     for (int64_t i = 0; i < np; ++i) out_h[dest[i]] = vals[i];
   }
+}
+
+int64_t Translator::ensure_score_slab() {
+  const int64_t V = mc_.tgt_vocab;
+  const size_t es = dtype_size(dtype_);
+  // row stride of the logits: the INT8 epilogue stores 16-byte rows (set_logits_ld)
+  const int64_t ld = projection_.kind == DenseWeights::INT8 ? (V + 7) / 8 * 8 : V;
+  if (!score_logits_.ptr) {
+    score_slab_rows_ = std::max<int64_t>(1, std::min<int64_t>(kScoreSlabRows, (static_cast<int64_t>(256) << 20) / (ld * es)));
+    score_logits_.alloc(static_cast<size_t>(score_slab_rows_) * ld * es);
+  }
+  return ld;
 }
 
 void Translator::encode(const int32_t* ids_h, const int32_t* lens_h, int64_t batch, int64_t S, float* memory_h) {
@@ -891,6 +911,215 @@ std::vector<TranslationHypotheses> Translator::whisper_generate(const WhisperReq
     CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));
   }
   return beam_.collect(bs, r.length_penalty, r.num_hypotheses, {}, stream_);
+}
+
+// =============================================================================================
+// Whisper::align and Whisper::detect_language
+// =============================================================================================
+namespace {
+constexpr int64_t kAlignScoreBytes = static_cast<int64_t>(256) << 20;   // captured scores of one pass (one entry at least)
+constexpr int64_t kDetectPassEntries = 16;                              // entries encoded at once by detect_language
+constexpr int64_t kAlignEncoderRows = 16 * 1500;                        // encoder rows of one pass: 16 windows of 30 s
+}  // namespace
+
+// WhisperReplica::align (whisper.cc:424-582) + compute_alignments (:387-422).  Entries are grouped into passes of at most
+// kScorePassRows decoder rows and kAlignScoreBytes of captured scores.  A pass runs the encoder and the memory projections, then
+// the decoder once over every input start + <|notimestamps|> + text + <|endoftext|> at positions 0 .. T - 1 (causal
+// self-attention; the memory is not masked), with the cross-attention of the alignment heads saving their scores.  The rows of
+// the text positions go through the final norm, the projection and SoftMax over [0, <|endoftext|>) + Gather.  The scores go
+// through SoftMax over the entry's frames, the standardisation of every frame column over the token rows (all T_max rows of
+// the batch when every entry has the same frame count -- the rows past an input's length are copies of its last row, as the
+// reference's Padder adds them back -- otherwise the entry's own rows), the median filter and the mean over the heads.  The
+// DTW matrices come back to the host, where negative_dtw runs.  Uncaptured; the search state is not touched.
+std::vector<WhisperAlignResult> Translator::whisper_align(const WhisperAlignRequest& r, float* matrix_h) {
+  std::lock_guard<std::mutex> lock(mu_);
+  CT2_REQUIRE(mc_.whisper, "whisper_align needs a Whisper model");
+  const int64_t B = r.batch, frames = r.frames, s0 = r.start_len, Nt = r.max_text;
+  const int64_t S = (frames + 2 - 3) / 2 + 1;
+  const int64_t V = mc_.tgt_vocab, d = mc_.d_model;
+  CT2_REQUIRE(B > 0 && frames >= 2 && S <= mc_.max_frames, "Invalid input features shape: too many frames for the encoder");
+  CT2_REQUIRE(s0 >= 1 && Nt >= 0, "align: the start sequence must not be empty");
+  CT2_REQUIRE(r.eot_id >= 1 && r.eot_id < V && r.no_timestamps_id >= 0 && r.no_timestamps_id < V, "align: special id out of range");
+  const int width = r.median_filter_width;
+  CT2_REQUIRE(width <= 1 || (width % 2 == 1 && width <= 129), "MedianFilter width must be odd and at most 129");
+  const int Hs = static_cast<int>(r.heads.size());
+  CT2_REQUIRE(Hs >= 1, "align: no alignment heads");
+  // layer order, then list order (set_alignment_heads, transformer.cc:577-584): slot k of layer l's list -> bit k of the mask
+  // of its head; layers without heads run the plain cross-attention
+  const int H = mc_.num_heads;
+  std::vector<int> count(mc_.dec_layers, 0);
+  std::vector<uint32_t> masks(static_cast<size_t>(mc_.dec_layers) * H, 0);
+  for (const auto& [layer, head] : r.heads) {
+    CT2_REQUIRE(layer >= 0 && layer < mc_.dec_layers && head >= 0 && head < H, "align: alignment head out of range");
+    CT2_REQUIRE(count[layer] < 32, "align: at most 32 alignment heads per layer");
+    masks[static_cast<size_t>(layer) * H + head] |= 1u << count[layer]++;
+  }
+  if (align_masks_.bytes < masks.size() * 4) align_masks_.alloc(masks.size() * 4);
+  CT2_CUDA_CHECK(cudaMemcpyAsync(align_masks_.ptr, masks.data(), masks.size() * 4, cudaMemcpyHostToDevice, stream_));
+  std::vector<AttnCapture> capture(mc_.dec_layers);
+  for (int l = 0, first = 0; l < mc_.dec_layers; ++l) {
+    capture[l].masks = count[l] ? align_masks_.as<uint32_t>() + static_cast<size_t>(l) * H : nullptr;
+    capture[l].first = first;
+    capture[l].total = Hs;
+    first += count[l];
+  }
+  for (int64_t t = 0; t < s0; ++t) CT2_REQUIRE(r.start[t] >= 0 && r.start[t] < V, "align: start id out of range");
+  std::vector<int32_t> nf(B), len(B);
+  int64_t Tg = 0;
+  bool all_zero = true, equal = true;
+  for (int64_t b = 0; b < B; ++b) {
+    CT2_REQUIRE(r.text_lens[b] >= 0 && r.text_lens[b] <= Nt, "align: text lengths must be in [0, max_text]");
+    for (int64_t t = 0; t < r.text_lens[b]; ++t)
+      CT2_REQUIRE(r.text[b * Nt + t] >= 0 && r.text[b * Nt + t] < V, "align: text id out of range");
+    CT2_REQUIRE(r.num_frames[b] >= 0, "align: num_frames must be >= 0");
+    nf[b] = r.num_frames[b] / 2;                      // the second convolution has stride 2
+    CT2_REQUIRE(nf[b] <= S, "align: num_frames exceeds the features' frames");
+    len[b] = static_cast<int32_t>(s0 + r.text_lens[b] + 2);
+    CT2_REQUIRE(len[b] <= dec_positions_, "No position encodings are defined for positions this far (common.cc:157-161)");
+    Tg = std::max<int64_t>(Tg, len[b]);
+    all_zero = all_zero && nf[b] == 0;
+    equal = equal && nf[b] == nf[0];
+  }
+  std::vector<WhisperAlignResult> results(B);
+  if (matrix_h) std::fill(matrix_h, matrix_h + B * (Nt + 1) * S, 0.f);
+  const size_t es = dtype_size(dtype_);
+  const int64_t ld = ensure_score_slab();
+  const float scale = 1.f / std::sqrt(static_cast<float>(mc_.head_dim));
+  for (int64_t p0 = 0; p0 < B;) {
+    int64_t p1 = p0 + 1, Tp = len[p0];
+    for (; p1 < B; ++p1) {
+      const int64_t t = std::max<int64_t>(Tp, len[p1]), n = p1 - p0 + 1;
+      if (n * t > kScorePassRows || n * S > kAlignEncoderRows || n * Hs * t * S * 4 > kAlignScoreBytes) break;
+      Tp = t;
+    }
+    const int64_t nb = p1 - p0, rows = nb * Tp;
+    // staged: decoder inputs [rows] | picked rows [np] | their text ids [np] | nf [nb] | len [nb] | text lengths [nb]
+    std::vector<int32_t> staged(rows, 0), picked, targets;
+    for (int64_t b = 0; b < nb; ++b) {
+      const int64_t g = p0 + b, n = r.text_lens[g];
+      int32_t* in = staged.data() + b * Tp;
+      std::copy(r.start, r.start + s0, in);
+      in[s0] = r.no_timestamps_id;
+      std::copy(r.text + g * Nt, r.text + g * Nt + n, in + s0 + 1);
+      in[s0 + 1 + n] = r.eot_id;
+      for (int64_t t = 0; t < n; ++t) {                 // logits at position s0 + t, gathered at text[t] (whisper.cc:495-502)
+        picked.push_back(static_cast<int32_t>(b * Tp + s0 + t));
+        targets.push_back(r.text[g * Nt + t]);
+      }
+    }
+    const int64_t np = static_cast<int64_t>(picked.size());
+    staged.insert(staged.end(), picked.begin(), picked.end());
+    staged.insert(staged.end(), targets.begin(), targets.end());
+    staged.insert(staged.end(), nf.begin() + p0, nf.begin() + p1);
+    staged.insert(staged.end(), len.begin() + p0, len.begin() + p1);
+    for (int64_t b = p0; b < p1; ++b) staged.push_back(r.text_lens[b]);
+    ensure_whisper_frontend(nb, S);
+    ensure_rows(nb, nb * S, std::max(rows, nb * S));
+    if (score_ids_.bytes < staged.size() * sizeof(int32_t)) score_ids_.alloc(staged.size() * sizeof(int32_t));
+    if (score_out_.bytes < std::max<int64_t>(np, 1) * sizeof(float)) score_out_.alloc(std::max<int64_t>(np, 1) * sizeof(float));
+    const size_t score_bytes = static_cast<size_t>(nb) * Hs * Tp * S * 4, norm_bytes = static_cast<size_t>(nb) * Hs * (Nt + 1) * S * 4;
+    const size_t matrix_bytes = static_cast<size_t>(nb) * (Nt + 1) * S * 4;
+    if (align_scores_.bytes < score_bytes) align_scores_.alloc(score_bytes);
+    if (align_norm_.bytes < norm_bytes) align_norm_.alloc(norm_bytes);
+    if (align_matrix_.bytes < matrix_bytes) align_matrix_.alloc(matrix_bytes);
+    const int32_t* dec_d = score_ids_.as<int32_t>();
+    const int32_t* picked_d = dec_d + rows;
+    const int32_t* targets_d = picked_d + np;
+    const int32_t* nf_d = targets_d + np;
+    const int32_t* len_d = nf_d + nb;
+    const int32_t* ntext_d = len_d + nb;
+    float* probs_d = score_out_.as<float>();
+    std::vector<int32_t> enc_lens(nb, static_cast<int32_t>(S));
+    CT2_CUDA_CHECK(cudaMemcpyAsync(features_.ptr, r.features + p0 * mc_.n_mels * frames, nb * mc_.n_mels * frames * 4,
+                                   cudaMemcpyHostToDevice, stream_));
+    CT2_CUDA_CHECK(cudaMemcpyAsync(src_lens_.ptr, enc_lens.data(), nb * 4, cudaMemcpyHostToDevice, stream_));
+    CT2_CUDA_CHECK(cudaMemcpyAsync(score_ids_.ptr, staged.data(), staged.size() * 4, cudaMemcpyHostToDevice, stream_));
+
+    run_whisper_encoder(nb, frames);
+    project_memory(nb, S);
+    for (auto& c : capture) c.out = align_scores_.as<float>();
+    launch_embed_pos(dec_emb_.weight.ptr, dec_emb_.kind == DenseWeights::INT8 ? dec_emb_.scale.as<float>() : nullptr, dec_d, rows, d,
+                     mc_.dec_emb_scale, dec_pos_.ptr, Tp, nullptr, false, x_.ptr, dtype_, stream_);
+    run_decoder_layers(rows, static_cast<int>(Tp), S, [&](int) {
+      launch_attention_causal(qkv_.ptr, nb, static_cast<int>(Tp), mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, dtype_, stream_);
+    }, &capture);
+    for (int64_t c = 0; c < np; c += score_slab_rows_) {
+      const int64_t k = std::min(score_slab_rows_, np - c);
+      launch_gather_rows(x_.ptr, picked_d + c, k, d * es, q_.ptr, stream_);
+      dense(projection_, mc_.has_dec_final_norm ? &dec_norm_ : nullptr, q_.ptr, k, nullptr, -1, score_logits_.ptr, false, ld);
+      launch_softmax_gather(score_logits_.ptr, targets_d + c, k, r.eot_id, ld, probs_d + c, dtype_, stream_);
+    }
+    std::vector<float> probs(np), matrix;
+    if (!all_zero) {
+      float* sc = align_scores_.as<float>();
+      launch_align_softmax(sc, nf_d, len_d, nb, Hs, Tp, S, dtype_, stream_);
+      launch_align_standardize(sc, nf_d, len_d, ntext_d, nb, Hs, Tp, S, equal ? Tg : 0, s0, Nt, S, align_norm_.as<float>(), dtype_,
+                               stream_);
+      launch_align_median_mean(align_norm_.as<float>(), nf_d, ntext_d, nb, Hs, Nt, S, width, align_matrix_.as<float>(), dtype_,
+                               stream_);
+      matrix.resize(nb * (Nt + 1) * S);
+      CT2_CUDA_CHECK(cudaMemcpyAsync(matrix.data(), align_matrix_.ptr, matrix_bytes, cudaMemcpyDeviceToHost, stream_));
+    }
+    if (np) CT2_CUDA_CHECK(cudaMemcpyAsync(probs.data(), probs_d, np * sizeof(float), cudaMemcpyDeviceToHost, stream_));
+    CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));     // also keeps the staging vectors alive until their copies are done
+    int64_t k = 0;
+    for (int64_t b = 0; b < nb; ++b) {
+      const int64_t g = p0 + b, n = r.text_lens[g];
+      results[g].text_token_probs.assign(probs.begin() + k, probs.begin() + k + n);
+      k += n;
+      if (all_zero || nf[g] == 0) continue;
+      const float* mb = matrix.data() + b * (Nt + 1) * S;
+      if (matrix_h) std::copy(mb, mb + (Nt + 1) * S, matrix_h + g * (Nt + 1) * S);
+      std::vector<float> x((n + 1) * nf[g]);
+      for (int64_t i = 0; i <= n; ++i) std::copy(mb + i * S, mb + i * S + nf[g], x.begin() + i * nf[g]);
+      results[g].path = negative_dtw(x.data(), n + 1, nf[g]);
+    }
+    p0 = p1;
+  }
+  return results;
+}
+
+// WhisperReplica::detect_language (whisper.cc:584-652): one decoder position per entry on <|startoftranscript|>, Gather of the
+// language ids' logits, SoftMax over them in T.  The caller sorts.
+void Translator::whisper_detect_language(const float* features_h, int64_t batch, int64_t frames, int32_t sot_id,
+                                         const std::vector<int32_t>& lang_ids, float* probs_h) {
+  std::lock_guard<std::mutex> lock(mu_);
+  CT2_REQUIRE(mc_.whisper, "detect_language needs a Whisper model");
+  const int64_t S = (frames + 2 - 3) / 2 + 1, V = mc_.tgt_vocab, d = mc_.d_model;
+  CT2_REQUIRE(batch > 0 && frames >= 2 && S <= mc_.max_frames, "Invalid input features shape: too many frames for the encoder");
+  CT2_REQUIRE(sot_id >= 0 && sot_id < V, "detect_language: <|startoftranscript|> out of range");
+  const int n = static_cast<int>(lang_ids.size());
+  CT2_REQUIRE(n >= 1, "detect_language: no language ids");
+  for (int32_t id : lang_ids) CT2_REQUIRE(id >= 0 && id < V, "detect_language: language id out of range");
+  const int64_t ld = ensure_score_slab();
+  const float scale = 1.f / std::sqrt(static_cast<float>(mc_.head_dim));
+  const int64_t per_pass = std::min<int64_t>(score_slab_rows_, kDetectPassEntries);
+  for (int64_t p0 = 0; p0 < batch; p0 += per_pass) {
+    const int64_t nb = std::min(per_pass, batch - p0);
+    ensure_whisper_frontend(nb, S);
+    ensure_rows(nb, nb * S, nb * S);
+    const size_t words = nb + n;                        // decoder inputs | language ids
+    if (score_ids_.bytes < words * sizeof(int32_t)) score_ids_.alloc(words * sizeof(int32_t));
+    if (score_out_.bytes < nb * n * sizeof(float)) score_out_.alloc(nb * n * sizeof(float));
+    std::vector<int32_t> staged(nb, sot_id), enc_lens(nb, static_cast<int32_t>(S));
+    staged.insert(staged.end(), lang_ids.begin(), lang_ids.end());
+    CT2_CUDA_CHECK(cudaMemcpyAsync(features_.ptr, features_h + p0 * mc_.n_mels * frames, nb * mc_.n_mels * frames * 4,
+                                   cudaMemcpyHostToDevice, stream_));
+    CT2_CUDA_CHECK(cudaMemcpyAsync(src_lens_.ptr, enc_lens.data(), nb * 4, cudaMemcpyHostToDevice, stream_));
+    CT2_CUDA_CHECK(cudaMemcpyAsync(score_ids_.ptr, staged.data(), staged.size() * 4, cudaMemcpyHostToDevice, stream_));
+    run_whisper_encoder(nb, frames);
+    project_memory(nb, S);
+    const int32_t* ids_d = score_ids_.as<int32_t>();
+    launch_embed_pos(dec_emb_.weight.ptr, dec_emb_.kind == DenseWeights::INT8 ? dec_emb_.scale.as<float>() : nullptr, ids_d, nb, d,
+                     mc_.dec_emb_scale, dec_pos_.ptr, 1, nullptr, false, x_.ptr, dtype_, stream_);
+    const bool xq = run_decoder_layers(nb, 1, S, [&](int) {
+      launch_attention_causal(qkv_.ptr, nb, 1, mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, dtype_, stream_);
+    });
+    dense(projection_, mc_.has_dec_final_norm ? &dec_norm_ : nullptr, x_.ptr, nb, nullptr, -1, score_logits_.ptr, xq, ld);
+    launch_gather_softmax(score_logits_.ptr, nb, ld, ids_d + nb, n, score_out_.as<float>(), dtype_, stream_);
+    CT2_CUDA_CHECK(cudaMemcpyAsync(probs_h + p0 * n, score_out_.ptr, nb * n * sizeof(float), cudaMemcpyDeviceToHost, stream_));
+    CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));
+  }
 }
 
 }  // namespace ct2b200

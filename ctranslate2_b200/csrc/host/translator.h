@@ -86,6 +86,26 @@ struct WhisperRequest {
   int max_initial_timestamp_index = 50;
   bool return_no_speech_prob = false;
 };
+// models::Whisper::align (include/ctranslate2/models/whisper.h:135-140, src/models/whisper.cc:424-582) on ids: every entry is
+// start + <|notimestamps|> + text + <|endoftext|>; heads = the (decoder layer, head) pairs of config.json's alignment_heads
+struct WhisperAlignRequest {
+  const float* features = nullptr;        // host [batch, n_mels, frames] f32
+  int64_t batch = 0, frames = 0;
+  const int32_t* start = nullptr;         // host [start_len]
+  int64_t start_len = 0;
+  const int32_t* text = nullptr;          // host [batch, max_text], right-padded
+  const int32_t* text_lens = nullptr;     // host [batch]
+  int64_t max_text = 0;
+  const int32_t* num_frames = nullptr;    // host [batch]: input frames of each entry (halved here, whisper.cc:505-509)
+  int median_filter_width = 7;
+  std::vector<std::pair<int, int>> heads;
+  int32_t no_timestamps_id = 0, eot_id = 0;
+};
+
+struct WhisperAlignResult {
+  std::vector<std::pair<int64_t, int64_t>> path;   // (text index, time index)
+  std::vector<float> text_token_probs;
+};
 
 
 class Translator {
@@ -111,6 +131,13 @@ class Translator {
              const int32_t* tgt_ids_h, const int32_t* tgt_lens_h, int64_t max_target_len, int64_t offset, float* out_h);
   // models::Whisper::generate; no_speech_h [batch] or null
   std::vector<TranslationHypotheses> whisper_generate(const WhisperRequest& req, float* no_speech_h);
+  // models::Whisper::align: one teacher-forced decoder pass per group of entries; matrix_h [batch, max_text + 1, (frames + 1)
+  // / 2] (the DTW input, zeros past each entry's rows and frames) or null.  Like score, it leaves the search state alone.
+  std::vector<WhisperAlignResult> whisper_align(const WhisperAlignRequest& req, float* matrix_h);
+  // models::Whisper::detect_language: probs_h [batch, lang_ids.size()] = SoftMax over the logits of lang_ids at the first
+  // decoder position (input <|startoftranscript|>), in lang_ids order
+  void whisper_detect_language(const float* features_h, int64_t batch, int64_t frames, int32_t sot_id,
+                               const std::vector<int32_t>& lang_ids, float* probs_h);
   // device-timed phases for bench.py: encoder pass, then `steps` decoding steps of batch * beam rows
   void bench(int64_t batch, int64_t source_len, int beam, int64_t steps, int64_t warmup, float* encode_ms, float* decode_ms,
              int64_t* launches);
@@ -121,6 +148,9 @@ class Translator {
   void drop_graph();            // synchronises and destroys the captured step (its buffers are about to move)
   void ensure_arena(int64_t batch, int64_t src_len, int beam, int64_t max_steps);
   void ensure_rows(int64_t entries, int64_t enc_rows, int64_t rows);
+  // the Whisper front-end buffers (features, im2col columns, convolution output) for `batch` windows of S encoder positions;
+  // the search state is not touched
+  void ensure_whisper_frontend(int64_t batch, int64_t S);
   // Dense on T rows (quantizes them for int8 weights); `pre` = the LayerNorm applied first (fused with the quantization)
   void dense(const DenseWeights& w, const NormWeights* pre, const void* x, int64_t rows, const void* residual, int act, void* y,
              bool prequantized = false, int64_t ldy = 0);
@@ -133,7 +163,11 @@ class Translator {
   void project_memory(int64_t batch, int64_t S);
   // the decoder layer stack on `rows` rows of x_; `self_attention(layer)` fills ctx_ from qkv_, and each run of
   // `rows_per_entry` rows attends to one memory entry.  Returns whether xq_ / xs_ hold Quantize(x_).
-  bool run_decoder_layers(int64_t rows, int rows_per_entry, int64_t S, const std::function<void(int)>& self_attention);
+  // `capture` (one entry per layer, count 0 = none): the cross-attention also saves the scores of those heads
+  bool run_decoder_layers(int64_t rows, int rows_per_entry, int64_t S, const std::function<void(int)>& self_attention,
+                          const std::vector<AttnCapture>* capture = nullptr);
+  // the score slab, allocated on first use; returns the row stride of its logits
+  int64_t ensure_score_slab();
   void decoder_step(int64_t rows, int beam, int64_t batch, int64_t S);
   void launch_or_capture_step(const BeamState& bs, int64_t S);
 
@@ -162,11 +196,14 @@ class Translator {
   BeamSearchArena beam_;         // search state: next ids, scores, histories, ancestry, hypotheses, counters
   DeviceBuffer features_, cols_, conv_out_, suppress_d_, forced_d_, no_speech_d_;   // Whisper
   int64_t cap_frames_ = 0;
+  int64_t cap_fe_batch_ = 0, cap_fe_src_ = 0;                    // Whisper front-end buffers
   int32_t* host_pinned_ = nullptr;
   size_t host_pinned_elems_ = 0;
   // score: logits slab [score_slab_rows_, vocab (padded)], per pass: decoder input ids | scored rows | their target ids, scores
   DeviceBuffer score_logits_, score_ids_, score_out_;
   int64_t score_slab_rows_ = 0;
+  // whisper_align: captured scores [entries, heads, T, S], standardised DTW rows [entries, heads, text + 1, S], DTW matrix
+  DeviceBuffer align_scores_, align_norm_, align_matrix_, align_masks_;
 
   cudaGraphExec_t graph_ = nullptr;
   int64_t graph_nodes_ = 0;

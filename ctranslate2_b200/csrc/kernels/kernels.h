@@ -34,6 +34,10 @@ void launch_softmax(const void* x, const int32_t* lengths, int64_t rows, int64_t
 // starts at x + r * ld (ld = 0: cols)
 void launch_log_softmax_gather(const void* x, const int32_t* ids, int64_t rows, int64_t cols, float* y, int dtype,
                                cudaStream_t st, int64_t ld = 0);
+// SoftMax over the first `cols` elements of a row + Gather, the same row reduction: y [rows] f32 = T(exp(x[r, ids[r]] -
+// logsumexp(x[r, :cols]))), 0 for an id outside [0, cols) (a masked softmax leaves 0 there); row r starts at x + r * ld
+void launch_softmax_gather(const void* x, const int32_t* ids, int64_t rows, int64_t cols, int64_t ld, float* y, int dtype,
+                           cudaStream_t st);
 void launch_topk(const void* x, int64_t rows, int64_t cols, int k, void* values, int32_t* indices, int dtype,
                  cudaStream_t st);
 
@@ -176,6 +180,17 @@ void launch_attention_beam_self(const void* qkv, void* k_cache, void* v_cache, c
                                 int64_t rows, int max_len, int H, int D, float scale, void* out, int dtype, cudaStream_t st);
 void launch_attention_cross(const void* q, const void* kv, const int32_t* lengths, int64_t rows, int beam, int S, int H, int D,
                             float scale, void* out, int dtype, cudaStream_t st);
+// The same cross-attention, also saving the pre-softmax scores T(scale * q.k) of selected heads (the attention a decoder
+// returns with return_normalized_attention() == false, attention.cc:267-270): row n = (entry n / beam, position n % beam);
+// masks [H] (device): bit k of masks[h] = head h goes to slot first + k of out [entries, total, beam, S] f32 (a head listed
+// twice is written twice).
+struct AttnCapture {
+  float* out = nullptr;
+  const uint32_t* masks = nullptr;
+  int first = 0, total = 0;
+};
+void launch_attention_cross_capture(const void* q, const void* kv, const int32_t* lengths, int64_t rows, int beam, int S, int H,
+                                    int D, float scale, void* out, const AttnCapture& cap, int dtype, cudaStream_t st);
 // causal self-attention of `time` teacher-forced decoder positions per sequence: qkv [batch * time, 3d] (row b * time + t
 // attends to rows b * time + j, j <= t), out [batch * time, d]; no cache is written
 void launch_attention_causal(const void* qkv, int64_t batch, int time, int H, int D, float scale, void* out, int dtype,
@@ -218,6 +233,24 @@ void launch_beam_force(const BeamState& s, const int32_t* forced_next, cudaStrea
 // out[r] = softmax(logits[r * row_stride : +vocab])[token]
 void launch_token_prob(const void* logits, int64_t rows, int64_t vocab, int64_t row_stride, int token, float* out, int dtype,
                        cudaStream_t st);
+// whisper_align.cu — models::Whisper::align post-processing (whisper.cc:387-560) and detect_language (:584-652).
+// scores [B, H, T, S] f32 (the captured T(scale * q.k)); nf [B] frames per entry (> 0 softmaxes), len [B] input lengths.
+// 1. SoftMax of every row t < len[b] over its first nf[b] frames, in place, rounded to T.
+void launch_align_softmax(float* scores, const int32_t* nf, const int32_t* len, int64_t batch, int heads, int64_t T, int64_t S,
+                          int dtype, cudaStream_t st);
+// 2. ops::LayerNorm(-2, 0) of every frame column over `rows` token rows (rows <= 0: len[b]; rows past len[b] - 1 read row
+//    len[b] - 1, the padding the reference's Padder adds back), written for the DTW rows start .. start + ntext[b] to
+//    norm [B, H, max_text + 1, F] f32 (T-rounded).
+void launch_align_standardize(const float* scores, const int32_t* nf, const int32_t* len, const int32_t* ntext, int64_t batch,
+                              int heads, int64_t T, int64_t S, int64_t rows, int64_t start, int64_t max_text, int64_t F,
+                              float* norm, int dtype, cudaStream_t st);
+// 3. ops::MedianFilter(width) along frames (mirrored edges; pass-through for width <= 1 or nf[b] <= width / 2), then
+//    ops::Mean over the heads: matrix [B, max_text + 1, F] f32 (T-rounded; zeros past nf[b] and past ntext[b] + 1 rows).
+void launch_align_median_mean(const float* norm, const int32_t* nf, const int32_t* ntext, int64_t batch, int heads,
+                              int64_t max_text, int64_t F, int width, float* matrix, int dtype, cudaStream_t st);
+// SoftMax over the logits of `n` ids (Gather then SoftMax, in T): probs [rows, n] f32 from rows of x at stride ld.
+void launch_gather_softmax(const void* x, int64_t rows, int64_t ld, const int32_t* ids, int n, float* probs, int dtype,
+                           cudaStream_t st);
 // ops::Conv1D as im2col (+ the float Dense): cols [batch * Tout, Cin * K] T from x [batch, Cin, Tin] (channel_major) or [batch, Tin, Cin]
 void launch_im2col(const void* x, bool x_is_f32, int64_t batch, int64_t Cin, int64_t Tin, int64_t Tout, int K, int stride,
                    int padding, bool channel_major, void* cols, int dtype, cudaStream_t st);

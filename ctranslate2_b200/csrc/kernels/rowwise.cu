@@ -303,7 +303,9 @@ __device__ __forceinline__ MaxSum warp_max_sum(MaxSum v) {
   return v;
 }
 
-template <typename T>
+// PROB: the probability T(exp(x[id] - logsumexp(x))) instead, 0 for an id outside the row (SoftMax over [0, cols) + Gather,
+// models/whisper.cc:495-502, where the mask leaves 0 past the limit).
+template <typename T, bool PROB = false>
 __global__ void __launch_bounds__(kRowThreads) log_softmax_gather_kernel(const T* __restrict__ x,
                                                                          const int32_t* __restrict__ ids, int64_t cols,
                                                                          int64_t ld, float* __restrict__ y) {
@@ -354,7 +356,8 @@ __global__ void __launch_bounds__(kRowThreads) log_softmax_gather_kernel(const T
       const int64_t id = ids[row];
       // an id outside the row has no log-probability: NaN rather than a read past the row
       const double v = static_cast<double>(to_f32(xr[id >= 0 && id < cols ? id : 0])) - acc.m - log(acc.s);
-      y[row] = id >= 0 && id < cols ? round_to<T>(static_cast<float>(v)) : NAN;
+      if constexpr (PROB) y[row] = id >= 0 && id < cols ? round_to<T>(static_cast<float>(exp(v))) : 0.f;
+      else y[row] = id >= 0 && id < cols ? round_to<T>(static_cast<float>(v)) : NAN;
     }
   }
 }
@@ -515,6 +518,15 @@ void launch_log_softmax_gather(const void* x, const int32_t* ids, int64_t rows, 
   if (rows == 0) return;
   CT2_DISPATCH_DTYPE(dtype, (log_softmax_gather_kernel<T><<<rows, kRowThreads, 0, st>>>(static_cast<const T*>(x), ids, cols,
                                                                                        ld > 0 ? ld : cols, y)));
+  check_launch();
+}
+
+void launch_softmax_gather(const void* x, const int32_t* ids, int64_t rows, int64_t cols, int64_t ld, float* y, int dtype,
+                           cudaStream_t st) {
+  if (rows == 0) return;
+  CT2_REQUIRE(cols >= 1 && ld >= cols, "softmax_gather: bad row width");
+  CT2_DISPATCH_DTYPE(dtype, (log_softmax_gather_kernel<T, true><<<rows, kRowThreads, 0, st>>>(static_cast<const T*>(x), ids, cols,
+                                                                                             ld, y)));
   check_launch();
 }
 

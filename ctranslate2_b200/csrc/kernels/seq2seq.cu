@@ -6,6 +6,7 @@
 // Reference kernels / functions these replace are cited per kernel (paths relative to the reference tree).
 #include <algorithm>
 #include <cfloat>
+#include <type_traits>
 
 #include "../common.cuh"
 #include "beam_decide.h"
@@ -191,12 +192,17 @@ struct AttnGeneric {
   bool vec_ok;               // every row start (q, k, v, caches, out) is 16-byte aligned
 };
 
+// the capture argument of the CAP instantiations; the others take an empty one, so their parameter block keeps its size
+struct NoCapture {};
+template <bool CAP> using CaptureArg = std::conditional_t<CAP, AttnCapture, NoCapture>;
+
 constexpr int kAttnWarps = 4;
 
 // DT = head_dim known at compile time (64, 128: the loops over a key / value row unroll, so the 16-byte loads of a row are all
-// in flight at once — with a run-time bound they are issued one L2 round trip at a time), 0 = any head_dim
-template <typename T, int MODE, int DT>
-__global__ void __launch_bounds__(kAttnWarps * 32) attention_generic_kernel(AttnGeneric a) {
+// in flight at once — with a run-time bound they are issued one L2 round trip at a time), 0 = any head_dim.  CAP: also write
+// the scores of the heads a.cap selects (Whisper::align); the other instantiations compile without it.
+template <typename T, int MODE, int DT, bool CAP = false>
+__global__ void __launch_bounds__(kAttnWarps * 32) attention_generic_kernel(AttnGeneric a, CaptureArg<CAP> cap) {
   extern __shared__ float smem_f[];
   griddep_launch();
   griddep_wait();
@@ -277,6 +283,8 @@ __global__ void __launch_bounds__(kAttnWarps * 32) attention_generic_kernel(Attn
     }
     return dot;
   };
+  uint32_t cap_mask = 0;     // CAP: the slots this head is saved to, read once per warp
+  if constexpr (CAP) cap_mask = cap.masks[h];
   // scores: one key per lane
   float m = -INFINITY;
   for (int j = lane; j < nkeys; j += 32) {
@@ -289,6 +297,11 @@ __global__ void __launch_bounds__(kAttnWarps * 32) attention_generic_kernel(Attn
     const float s = round_to<T>(dot * a.scale);
     sc[j] = s;
     m = fmaxf(m, s);
+    if constexpr (CAP) {
+      const int64_t e = n / a.beam, t = n - e * a.beam;
+      for (uint32_t mk = cap_mask; mk; mk &= mk - 1)
+        cap.out[((e * cap.total + cap.first + __ffs(mk) - 1) * a.beam + t) * a.S + j] = s;
+    }
   }
   m = warp_max(m);
   float sum = 0.f;
@@ -875,8 +888,8 @@ void launch_layer_norm(const void* x, const void* gamma, const void* beta, int64
 }
 
 namespace {
-template <typename T, int MODE>
-void launch_attn_mode(const AttnGeneric& a_in, cudaStream_t st) {
+template <typename T, int MODE, bool CAP = false>
+void launch_attn_mode(const AttnGeneric& a_in, cudaStream_t st, const CaptureArg<CAP>& cap = {}) {
   AttnGeneric a = a_in;
   {
     const size_t es = sizeof(T);
@@ -886,14 +899,14 @@ void launch_attn_mode(const AttnGeneric& a_in, cudaStream_t st) {
   }
   const size_t smem = static_cast<size_t>(kAttnWarps) * (a.max_keys + a.D) * sizeof(float);
   CT2_REQUIRE(smem <= 200 * 1024, "attention: too many keys for the generic kernel");
-  auto kernel = a.D == 64 ? attention_generic_kernel<T, MODE, 64>
-                : a.D == 128 ? attention_generic_kernel<T, MODE, 128> : attention_generic_kernel<T, MODE, 0>;
+  auto kernel = a.D == 64 ? attention_generic_kernel<T, MODE, 64, CAP>
+                : a.D == 128 ? attention_generic_kernel<T, MODE, 128, CAP> : attention_generic_kernel<T, MODE, 0, CAP>;
   if (smem > 48 * 1024) {
     // the attribute is per device: set it whenever the request grows (cheap, idempotent)
     CT2_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   }
   const int64_t units = a.rows * a.H;
-  launch_pdl(kernel, dim3(static_cast<unsigned>((units + kAttnWarps - 1) / kAttnWarps)), dim3(kAttnWarps * 32), smem, st, a);
+  launch_pdl(kernel, dim3(static_cast<unsigned>((units + kAttnWarps - 1) / kAttnWarps)), dim3(kAttnWarps * 32), smem, st, a, cap);
   check_launch();
 }
 }  // namespace
@@ -991,6 +1004,31 @@ void launch_attention_cross(const void* q, const void* kv, const int32_t* length
   a.scale = scale;
   a.max_keys = S;
   CT2_DISPATCH_DTYPE(dtype, (launch_attn_mode<T, 2>(a, st)));
+}
+
+void launch_attention_cross_capture(const void* q, const void* kv, const int32_t* lengths, int64_t rows, int beam, int S, int H,
+                                    int D, float scale, void* out, const AttnCapture& cap, int dtype, cudaStream_t st) {
+  if (rows == 0) return;
+  CT2_REQUIRE(cap.out && cap.masks && cap.first >= 0 && cap.first < cap.total, "attention capture: bad heads");
+  const int64_t d = static_cast<int64_t>(H) * D;
+  const size_t es = dtype_size(dtype);
+  AttnGeneric a{};
+  a.q = q;
+  a.q_stride = d;
+  a.k = kv;
+  a.v = static_cast<const uint8_t*>(kv) + d * es;
+  a.kv_stride = 2 * d;
+  a.out = out;
+  a.out_stride = d;
+  a.lengths = lengths;
+  a.rows = rows;
+  a.S = S;
+  a.beam = beam;
+  a.H = H;
+  a.D = D;
+  a.scale = scale;
+  a.max_keys = S;
+  CT2_DISPATCH_DTYPE(dtype, (launch_attn_mode<T, 2, true>(a, st, cap)));
 }
 
 void launch_beam_init(void* cum, int32_t* ids, int64_t rows, int beam, int start_id, int dtype, cudaStream_t st) {

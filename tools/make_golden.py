@@ -381,8 +381,117 @@ def make_whisper_fixture():
     print("whisper fixture:", sum(len(m["cases"]) for m in fixture["models"].values()), "cases")
 
 
+WHISPER_ALIGN_HEADS = [[1, 2], [0, 1], [1, 0]]   # both decoder layers, out of order: the copy's config.json
+
+
+def whisper_align_cases():
+    """(seed, batch, start_sequence, text rows, num_frames, median_filter_width) on tiny_whisper (60 input frames = 30
+    encoder positions, 64 decoder positions; ids: text < 100, <|endoftext|> 100, <|startoftranscript|> 101, languages
+    102-104, <|transcribe|> 106, <|notimestamps|> 110)."""
+    rng = np.random.default_rng(33)
+    text = lambda n: [int(x) for x in rng.integers(0, 100, size=n)]   # noqa: E731
+    sot3, sot1 = [101, 102, 106], [101]
+    return [
+        (400, 1, sot3, [text(5)], [60], 7),                                        # one entry, equal full frames
+        (401, 2, sot3, [text(4), text(9)], [60, 60], 7),                             # ragged texts, equal full frames
+        (402, 3, sot1, [[], text(1), text(6)], [40, 40, 40], 3),                     # empty and one-token texts, partial
+        (403, 4, sot3, [text(3), text(7), text(2), text(5)], [41, 41, 41, 41], 7),  # odd frame count
+        (404, 4, sot3, [text(6), text(3), text(8), text(4)], [60, 3, 0, 37], 7),    # variable frames with 1 and 0
+        (405, 2, sot1, [text(5), text(2)], [1, 0], 7),                               # all below 2: empty alignments
+        (406, 2, sot3, [text(59), text(10)], [60, 50], 7),                           # fills the 64 positions, variable
+        (407, 2, sot3, [text(59), text(3)], [60, 60], 3),                            # fills the 64 positions, equal
+        (408, 3, sot3, [text(4), text(8), text(2)], [60, 44, 60], 1),                # width 1: pass-through
+        (409, 2, sot1, [text(6), text(3)], [40, 40], 61),                            # wider than the frames
+        (410, 2, sot3, [text(3) + [100, 105] + text(2), text(4)], [60, 60], 7),     # ids >= <|endoftext|> in a text
+        (411, 3, sot1, [text(7), text(1), text(12)], [24, 58, 33], 3),               # variable, width 3
+    ]
+
+
+def _ref_whisper_align(model_dir, compute, requests):
+    """models::Whisper::align / detect_language of the unmodified reference (CPU) through tools/ref_whisper_align.cc, built by
+    tools/ref_whisper_align.mk against oracle/_ref/libct2ref.so into a temporary directory."""
+    import subprocess
+    import tempfile
+    out_dir = os.path.join(tempfile.gettempdir(), "ct2ref_align")
+    subprocess.run(["make", "-s", "-f", "tools/ref_whisper_align.mk", "align", "ALIGN_OUT=" + out_dir], cwd=ROOT, check=True)
+    lines, counts = [], []
+    for i, req in enumerate(requests):
+        path = os.path.join(out_dir, "features_%d.f32" % i)
+        req["features"].astype(np.float32).tofile(path)
+        dims = " ".join(str(x) for x in req["features"].shape)
+        if req["kind"] == "align":
+            lines.append("\t".join(["align", path, dims, str(req["width"]), " ".join(map(str, req["start"])),
+                                    ";".join(" ".join(map(str, t)) for t in req["text"]), " ".join(map(str, req["num_frames"]))]))
+        else:
+            lines.append("\t".join(["lang", path, dims]))
+        counts.append(req["features"].shape[0])
+    text = "%s\t%s\n" % (model_dir, compute) + "".join(x + "\n" for x in lines)
+    out = subprocess.run([os.path.join(out_dir, "ref_whisper_align")], input=text.encode(), capture_output=True,
+                         check=True).stdout.decode().split("\n")
+    res, k = [], 0
+    for req, n in zip(requests, counts):
+        assert out[k] == "ok", out[k]
+        rows = out[k + 1:k + 1 + n]
+        k += 1 + n
+        if req["kind"] == "align":
+            entries = []
+            for r in rows:
+                a, p = r.split("\t")
+                entries.append({"alignments": [[int(x) for x in pair.split(",")] for pair in a.split(" ")] if a else [],
+                                "text_token_probs": [float(x) for x in p.split(" ")] if p else []})
+            res.append(entries)
+        else:
+            res.append([[(t, float(v)) for t, v in zip(r.split(" ")[0::2], r.split(" ")[1::2])] for r in rows])
+    return res
+
+
+def make_whisper_align_fixture():
+    """models::Whisper::align and ::detect_language of the UNMODIFIED reference (oracle/_ref, CPU) on tiny_whisper, in float32
+    and int8: with the model's own alignment_heads, and with a temporary copy whose config.json lists heads of both layers out
+    of order (WHISPER_ALIGN_HEADS; the tests recreate the copy).  Features are re-generated from their seeds."""
+    import shutil
+    import tempfile
+    src = os.path.join(OUT, "tiny_whisper")
+    tmp = tempfile.mkdtemp()
+    permuted = os.path.join(tmp, "tiny_whisper_heads")
+    shutil.copytree(src, permuted)
+    cfg = json.load(open(os.path.join(src, "config.json")))
+    cfg["alignment_heads"] = WHISPER_ALIGN_HEADS
+    json.dump(cfg, open(os.path.join(permuted, "config.json"), "w"))
+    # this reference calls a model multilingual when its vocabulary holds the empty token (whisper.cc:72): a second copy
+    # renames the unused text token <t99> for detect_language
+    multilingual = os.path.join(tmp, "tiny_whisper_multilingual")
+    shutil.copytree(src, multilingual)
+    vocab = json.load(open(os.path.join(src, "vocabulary.json"), encoding="utf-8"))
+    vocab[99] = ""
+    json.dump(vocab, open(os.path.join(multilingual, "vocabulary.json"), "w", encoding="utf-8"))
+    fixture = {"n_mels": 16, "frames": 60, "permuted_heads": WHISPER_ALIGN_HEADS, "models": {}}
+    lang_seeds = [(420, 3), (421, 1)]
+    for heads, mdir in (("model", src), ("permuted", permuted)):
+        for compute in ("float32", "int8"):
+            reqs = [{"kind": "align", "features": whisper_inputs(seed, batch, 16, 60), "start": start, "text": text,
+                     "num_frames": nf, "width": width} for seed, batch, start, text, nf, width in whisper_align_cases()]
+            res = _ref_whisper_align(mdir, compute, reqs)
+            cases = [{"seed": seed, "batch": batch, "start_sequence": start, "text_tokens": text, "num_frames": nf,
+                      "median_filter_width": width, "results": r}
+                     for (seed, batch, start, text, nf, width), r in zip(whisper_align_cases(), res)]
+            entry = {"heads": heads, "compute_type": compute, "cases": cases}
+            if heads == "model":
+                res = _ref_whisper_align(multilingual, compute, [{"kind": "lang", "features": whisper_inputs(seed, batch, 16, 60)}
+                                                                  for seed, batch in lang_seeds])
+                entry["detect_language"] = [{"seed": seed, "batch": batch, "results": r} for (seed, batch), r in zip(lang_seeds, res)]
+            fixture["models"]["%s-%s" % (heads, compute)] = entry
+    shutil.rmtree(tmp)
+    with open(os.path.join(OUT, "whisper_align_ref.json"), "w") as f:
+        json.dump(fixture, f)
+    print("whisper align fixture:", sum(len(m["cases"]) for m in fixture["models"].values()), "cases")
+
+
 def main():
     os.makedirs(OUT, exist_ok=True)
+    if "--whisper-align-only" in sys.argv:
+        make_whisper_align_fixture()
+        return
     if "--scores-only" in sys.argv:
         make_scores_fixture()
         return
@@ -474,6 +583,7 @@ def main():
     make_seq2seq_fixture()
     make_translator_score_fixture()
     make_whisper_fixture()
+    make_whisper_align_fixture()
     print("done")
 
 
