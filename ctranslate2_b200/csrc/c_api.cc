@@ -276,6 +276,73 @@ CT2B200_API int ct2b200_attention_prefill(const void* qkv, void* k_cache, void* 
   });
 }
 
+CT2B200_API int ct2b200_attention_encoder(const void* qkv, const int32_t* lengths, int64_t batch, int keys, int H, int D,
+                                          float scale, void* out, int dtype, void* stream) {
+  return guarded([&] {
+    require_device();
+    CT2_REQUIRE(batch >= 0 && keys >= 0 && H > 0 && D > 0, "attention_encoder: bad shape");
+    launch_attention_encoder(qkv, lengths, batch, keys, H, D, scale, out, dtype, S(stream));
+  });
+}
+
+CT2B200_API int ct2b200_attention_causal(const void* qkv, int64_t batch, int time, int H, int D, float scale, void* out, int dtype,
+                                         void* stream) {
+  return guarded([&] {
+    require_device();
+    CT2_REQUIRE(batch >= 0 && time >= 0 && H > 0 && D > 0, "attention_causal: bad shape");
+    launch_attention_causal(qkv, batch, time, H, D, scale, out, dtype, S(stream));
+  });
+}
+
+CT2B200_API int ct2b200_attention_beam_self(const void* qkv, void* k_cache, void* v_cache, const int32_t* anc, const int32_t* step_d,
+                                            int64_t rows, int max_len, int H, int D, float scale, void* out, int dtype,
+                                            void* stream) {
+  return guarded([&] {
+    require_device();
+    CT2_REQUIRE(rows >= 0 && max_len > 0 && H > 0 && D > 0, "attention_beam_self: bad shape");
+    launch_attention_beam_self(qkv, k_cache, v_cache, anc, step_d, rows, max_len, H, D, scale, out, dtype, S(stream));
+  });
+}
+
+CT2B200_API int ct2b200_attention_cross(const void* q, const void* kv, const int32_t* lengths, int64_t rows, int beam, int keys,
+                                        int H, int D, float scale, void* out, float* capture_out, const uint32_t* masks_d, int first,
+                                        int total, int dtype, void* stream) {
+  return guarded([&] {
+    require_device();
+    CT2_REQUIRE(rows >= 0 && beam > 0 && rows % beam == 0 && keys >= 0 && H > 0 && D > 0, "attention_cross: bad shape");
+    if (!capture_out) {
+      launch_attention_cross(q, kv, lengths, rows, beam, keys, H, D, scale, out, dtype, S(stream));
+      return;
+    }
+    AttnCapture cap;
+    cap.out = capture_out;
+    cap.masks = masks_d;
+    cap.first = first;
+    cap.total = total;
+    launch_attention_cross_capture(q, kv, lengths, rows, beam, keys, H, D, scale, out, cap, dtype, S(stream));
+  });
+}
+
+CT2B200_API int ct2b200_beam_rows(void* logits, const void* cum, int32_t* step_d, int batch, int beam, int vocab, int64_t vocab_ld,
+                                  int min_length, const int32_t* end_ids_d, int num_end, void* row_scores, int32_t* row_ids,
+                                  int dtype, void* stream) {
+  return guarded([&] {
+    require_device();
+    CT2_REQUIRE(batch >= 0 && vocab > 0 && vocab_ld >= vocab && num_end >= 0 && (num_end == 0 || end_ids_d),
+                "beam_rows: bad shape");
+    BeamState s;
+    s.batch = batch;
+    s.beam = beam;
+    s.vocab = vocab;
+    s.vocab_ld = vocab_ld;
+    s.min_length = min_length;
+    s.end_ids = end_ids_d;
+    s.num_end = num_end;
+    s.step = step_d;
+    launch_beam_rows(logits, cum, s, row_scores, row_ids, dtype, S(stream));
+  });
+}
+
 CT2B200_API int ct2b200_awq_repack(const int32_t* qweight, const void* scales, const int32_t* qzeros, int layout, int group_size,
                        int64_t n, int64_t k, int32_t* wp, void* sc, void* zr, void* sz, void* stream) {
   return guarded([&] {

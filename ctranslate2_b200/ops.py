@@ -327,6 +327,84 @@ def attention_prefill(qkv, k_cache, v_cache, sin, cos, batch, time, offset, num_
     return out
 
 
+# ---------------- encoder-decoder attention and the beam-search row step (seq2seq.cu) ----------------
+# Inputs are used where they lie (no copy), so that callers can pass views at any element offset; rows must be contiguous.
+def _rows(t: torch.Tensor) -> torch.Tensor:
+    if not t.is_cuda:
+        raise ValueError("ctranslate2_b200 ops run on Device::CUDA only (no CPU fallback)")
+    if not t.is_contiguous():
+        raise ValueError("rows must be contiguous")
+    return t
+
+
+def attention_encoder(qkv, num_heads, head_dim, batch, lengths=None, scale=None):
+    """Encoder self-attention with a padding mask: qkv [batch * S, 3d] -> out [batch * S, d]; lengths int32 [batch] or None."""
+    qkv = _rows(qkv)
+    d = num_heads * head_dim
+    S = qkv.shape[0] // batch if batch else 0
+    scale = head_dim ** -0.5 if scale is None else scale
+    out = torch.empty((batch * S, d), dtype=qkv.dtype, device=qkv.device)
+    check(lib().ct2b200_attention_encoder(_p(qkv), _p(lengths), ctypes.c_int64(batch), S, num_heads, head_dim,
+                                          ctypes.c_float(scale), _p(out), _dt(qkv), _stream()))
+    return out
+
+
+def attention_causal(qkv, num_heads, head_dim, batch, scale=None):
+    """Teacher-forced causal self-attention: qkv [batch * time, 3d] -> out [batch * time, d]."""
+    qkv = _rows(qkv)
+    d = num_heads * head_dim
+    time = qkv.shape[0] // batch if batch else 0
+    scale = head_dim ** -0.5 if scale is None else scale
+    out = torch.empty((batch * time, d), dtype=qkv.dtype, device=qkv.device)
+    check(lib().ct2b200_attention_causal(_p(qkv), ctypes.c_int64(batch), time, num_heads, head_dim, ctypes.c_float(scale),
+                                         _p(out), _dt(qkv), _stream()))
+    return out
+
+
+def attention_beam_self(qkv, k_cache, v_cache, anc, step, num_heads, head_dim, scale=None):
+    """One-token decoder self-attention over the beam-remapped cache: qkv [rows, 3d]; k_cache / v_cache [rows, max_len, d]
+    (the rows' new k / v are written at position step); anc int32 [2, rows, max_len]; step: int32 [1] device tensor."""
+    qkv, k_cache, v_cache, anc = _rows(qkv), _rows(k_cache), _rows(v_cache), _rows(anc)
+    rows, max_len = k_cache.shape[0], k_cache.shape[1]
+    scale = head_dim ** -0.5 if scale is None else scale
+    out = torch.empty((rows, num_heads * head_dim), dtype=qkv.dtype, device=qkv.device)
+    check(lib().ct2b200_attention_beam_self(_p(qkv), _p(k_cache), _p(v_cache), _p(anc), _p(step), ctypes.c_int64(rows), max_len,
+                                            num_heads, head_dim, ctypes.c_float(scale), _p(out), _dt(qkv), _stream()))
+    return out
+
+
+def attention_cross(q, kv, num_heads, head_dim, beam, lengths=None, scale=None, capture=None, masks=None, first=0,
+                    total=0):
+    """Cross-attention: q [rows, d], kv [batch * S, 2d] with batch = rows / beam -> out [rows, d].  capture (float32
+    [batch, total, beam, S]) with masks (uint32 as int32 [H]): also save the scores of the selected heads."""
+    q, kv = _rows(q), _rows(kv)
+    rows = q.shape[0]
+    batch = rows // beam
+    S = kv.shape[0] // batch if batch else 0
+    scale = head_dim ** -0.5 if scale is None else scale
+    out = torch.empty((rows, num_heads * head_dim), dtype=q.dtype, device=q.device)
+    check(lib().ct2b200_attention_cross(_p(q), _p(kv), _p(lengths), ctypes.c_int64(rows), beam, S, num_heads, head_dim,
+                                        ctypes.c_float(scale), _p(out), _p(capture), _p(masks), first, total, _dt(q),
+                                        _stream()))
+    return out
+
+
+def beam_rows(logits, cum, step, beam, vocab, min_length=0, end_ids=None):
+    """One beam-search step of every row: logits [batch * beam, vocab_ld] in T (the end ids are disabled in place while
+    step < min_length), cum [batch * beam] T, step int32 [1] device tensor -> (scores T, ids int32) [batch * beam, 2 * beam],
+    ids flattened over [beam, vocab]."""
+    if beam < 1:
+        raise ValueError("beam_rows: beam_size must be in [1, 8]")
+    logits, cum = _rows(logits), _rows(cum)
+    rows, vocab_ld = logits.shape
+    num_end = 0 if end_ids is None else int(end_ids.numel())
+    scores = torch.empty((rows, 2 * beam), dtype=logits.dtype, device=logits.device)
+    ids = torch.empty((rows, 2 * beam), dtype=torch.int32, device=logits.device)
+    check(lib().ct2b200_beam_rows(_p(logits), _p(cum), _p(step), rows // beam, beam, vocab, ctypes.c_int64(vocab_ld), min_length,
+                                  _p(end_ids), num_end, _p(scores), _p(ids), _dt(logits), _stream()))
+    return scores, ids
+
+
 # ---------------- AWQ-INT4 (ops::GemmAwq / GemvAwq / DequantizeAwq) ----------------
 AWQ_GEMM, AWQ_GEMV = 1, 2
 

@@ -196,6 +196,45 @@ CT2B200_API int ct2b200_attention_prefill(const void* qkv_d, void* k_cache_d, vo
                               int rotary_interleave, float scale, void* out_d, int dtype, void* stream);
 
 /* ---------------------------------------------------------------------------------------------
+ * Encoder-decoder attention (layers::MultiHeadAttention of TransformerEncoder / TransformerDecoder, dot_product_attention,
+ * src/layers/attention.cc:178-287): the kernel the Translator and Whisper run, exposed op by op.  Any head_dim; one warp per
+ * (query row, head); scores T(scale * q.k), probabilities T(softmax), context T(sum p.v).  d = H * D, every row is T.
+ * These calls fail with "invalid argument" when the per-warp score buffer (4 * (keys + D) floats) would exceed 200 KB.
+ * ------------------------------------------------------------------------------------------- */
+
+/* Encoder self-attention: qkv_d [batch * S, 3d] ([q | k | v]); row (b, t) attends to rows (b, j), j < lengths_d[b]
+ * (NULL = S; a length of 0 gives a zero row).  out_d [batch * S, d]. */
+CT2B200_API int ct2b200_attention_encoder(const void* qkv_d, const int32_t* lengths_d, int64_t batch, int S, int H, int D,
+                                          float scale, void* out_d, int dtype, void* stream);
+/* Teacher-forced causal decoder self-attention: qkv_d [batch * time, 3d]; row (b, t) attends to rows (b, j), j <= t.
+ * out_d [batch * time, d]. */
+CT2B200_API int ct2b200_attention_causal(const void* qkv_d, int64_t batch, int time, int H, int D, float scale, void* out_d,
+                                         int dtype, void* stream);
+/* One-token decoder self-attention over a beam-remapped cache: k_cache_d / v_cache_d [rows, max_len, d];
+ * anc_d int32 [2][rows, max_len] (the table of parity *step_d & 1 is read); key j < step of row n lives at
+ * (anc[n][j], j).  The row's new k / v (columns d.. and 2d.. of qkv_d [rows, 3d]) are written to (n, step).
+ * step_d: int32 [1] on the device, step < max_len.  out_d [rows, d]. */
+CT2B200_API int ct2b200_attention_beam_self(const void* qkv_d, void* k_cache_d, void* v_cache_d, const int32_t* anc_d,
+                                            const int32_t* step_d, int64_t rows, int max_len, int H, int D, float scale,
+                                            void* out_d, int dtype, void* stream);
+/* Cross-attention: q_d [rows, d]; kv_d [batch * S, 2d] ([k | v]) with batch = rows / beam; row n attends to the first
+ * lengths_d[n / beam] (NULL = S) rows of entry n / beam.  out_d [rows, d].  capture_out_d NULL: plain cross-attention.
+ * Otherwise the scores T(scale * q.k) of the selected heads are also written, as f32, to
+ * capture_out_d [batch, total, beam, S]: bit k of masks_d[h] (uint32 [H], device) sends head h to slot first + k, which must
+ * be below total; positions at or past the entry's length are not written. */
+CT2B200_API int ct2b200_attention_cross(const void* q_d, const void* kv_d, const int32_t* lengths_d, int64_t rows, int beam,
+                                        int S, int H, int D, float scale, void* out_d, float* capture_out_d,
+                                        const uint32_t* masks_d, int first, int total, int dtype, void* stream);
+/* One beam-search step of every row (BeamSearch::search, src/decoding.cc:425-720): end ids disabled while *step_d <
+ * min_length (in place in logits_d), LogSoftMax, + cum_d[row], then the row's best 2 * beam candidates ordered by
+ * (score desc, index asc), ids flattened over [beam, vocab] (row % beam) and (-inf, -1) past the vocabulary.
+ * logits_d [batch * beam, vocab_ld] T; cum_d [batch * beam] T; row_scores_d T / row_ids_d int32 [batch * beam, 2 * beam].
+ * beam must be in [1, 8]. */
+CT2B200_API int ct2b200_beam_rows(void* logits_d, const void* cum_d, int32_t* step_d, int batch, int beam, int vocab,
+                                  int64_t vocab_ld, int min_length, const int32_t* end_ids_d, int num_end, void* row_scores_d,
+                                  int32_t* row_ids_d, int dtype, void* stream);
+
+/* ---------------------------------------------------------------------------------------------
  * AWQ-INT4 (SURVEY §8 a7): ops::GemmAwq / GemvAwq / DequantizeAwq — include/ctranslate2/ops/awq/{gemm,gemv,dequantize}.h,
  * src/ops/awq/{gemm,gemv,dequantize}_gpu.cu.  x [m,k] f16 -> y [m,n] f16.
  * layout 1 = AWQ_GEMM: qweight int32 [k, n/8], scales f16 [k/g, n], qzeros int32 [k/g, n/8]
