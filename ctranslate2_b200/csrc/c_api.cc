@@ -43,6 +43,21 @@ void require_device() {
   if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0)
     throw std::runtime_error("no CUDA device: ct2b200 has no CPU fallback");
 }
+
+// the num_hypotheses best hypotheses of every entry: out_ids [batch, num_hypotheses, max_length] (-1 padded), out_lens and
+// out_scores [batch, num_hypotheses] (-1 and 0 for a hypothesis an entry does not have)
+void copy_hypotheses(const std::vector<TranslationHypotheses>& res, int64_t batch, int num_hypotheses, int64_t max_length,
+                     int32_t* out_ids, int32_t* out_lens, float* out_scores) {
+  for (int64_t b = 0; b < batch; ++b)
+    for (int h = 0; h < num_hypotheses; ++h) {
+      int32_t* dst = out_ids + (b * num_hypotheses + h) * max_length;
+      const bool have = h < static_cast<int>(res[b].tokens.size());
+      const int64_t len = have ? static_cast<int64_t>(res[b].tokens[h].size()) : 0;
+      for (int64_t i = 0; i < max_length; ++i) dst[i] = i < len ? res[b].tokens[h][i] : -1;
+      out_lens[b * num_hypotheses + h] = have ? static_cast<int32_t>(len) : -1;
+      out_scores[b * num_hypotheses + h] = have ? res[b].scores[h] : 0.f;
+    }
+}
 }  // namespace
 
 struct ct2b200_generator {
@@ -476,16 +491,7 @@ CT2B200_API int ct2b200_generate_batch_beam(ct2b200_generator* g, const int32_t*
     r.patience = patience;
     r.length_penalty = length_penalty;
     r.num_hypotheses = num_hypotheses;
-    const std::vector<TranslationHypotheses> res = g->impl->generate_beam(r);
-    for (int64_t b = 0; b < batch; ++b)
-      for (int h = 0; h < num_hypotheses; ++h) {
-        int32_t* dst = out_ids + (b * num_hypotheses + h) * max_length;
-        const bool have = h < static_cast<int>(res[b].tokens.size());
-        const int64_t len = have ? static_cast<int64_t>(res[b].tokens[h].size()) : 0;
-        for (int64_t i = 0; i < max_length; ++i) dst[i] = i < len ? res[b].tokens[h][i] : -1;
-        out_lens[b * num_hypotheses + h] = have ? static_cast<int32_t>(len) : -1;
-        out_scores[b * num_hypotheses + h] = have ? res[b].scores[h] : 0.f;
-      }
+    copy_hypotheses(g->impl->generate_beam(r), batch, num_hypotheses, max_length, out_ids, out_lens, out_scores);
   });
 }
 
@@ -652,16 +658,7 @@ CT2B200_API int ct2b200_translate_batch(ct2b200_translator* t, const int32_t* so
     r.start_id = start_id;
     r.end_ids.assign(end_ids, end_ids + (end_ids ? num_end_ids : 0));
     r.return_end_token = return_end_token != 0;
-    const std::vector<TranslationHypotheses> res = t->impl->translate(r);
-    for (int64_t b = 0; b < batch; ++b)
-      for (int h = 0; h < num_hypotheses; ++h) {
-        int32_t* dst = out_ids + (b * num_hypotheses + h) * max_decoding_length;
-        const bool have = h < static_cast<int>(res[b].tokens.size());
-        const int64_t len = have ? static_cast<int64_t>(res[b].tokens[h].size()) : 0;
-        for (int64_t i = 0; i < max_decoding_length; ++i) dst[i] = i < len ? res[b].tokens[h][i] : -1;
-        out_lens[b * num_hypotheses + h] = have ? static_cast<int32_t>(len) : -1;
-        out_scores[b * num_hypotheses + h] = have ? res[b].scores[h] : 0.f;
-      }
+    copy_hypotheses(t->impl->translate(r), batch, num_hypotheses, max_decoding_length, out_ids, out_lens, out_scores);
   });
 }
 
@@ -760,16 +757,7 @@ CT2B200_API int ct2b200_whisper_generate(ct2b200_translator* t, const float* fea
     r.no_speech_id = no_speech_id;
     r.no_timestamps_id = no_timestamps_id;
     r.max_initial_timestamp_index = max_initial_timestamp_index;
-    const std::vector<TranslationHypotheses> res = t->impl->whisper_generate(r, no_speech);
-    for (int64_t b = 0; b < batch; ++b)
-      for (int h = 0; h < num_hypotheses; ++h) {
-        int32_t* dst = out_ids + (b * num_hypotheses + h) * max_length;
-        const bool have = h < static_cast<int>(res[b].tokens.size());
-        const int64_t len = have ? static_cast<int64_t>(res[b].tokens[h].size()) : 0;
-        for (int64_t i = 0; i < max_length; ++i) dst[i] = i < len ? res[b].tokens[h][i] : -1;
-        out_lens[b * num_hypotheses + h] = have ? static_cast<int32_t>(len) : -1;
-        out_scores[b * num_hypotheses + h] = have ? res[b].scores[h] : 0.f;
-      }
+    copy_hypotheses(t->impl->whisper_generate(r, no_speech), batch, num_hypotheses, max_length, out_ids, out_lens, out_scores);
   });
 }
 

@@ -187,6 +187,46 @@ void DeviceBuffer::release() {
   bytes = 0;
 }
 
+void StepGraph::reset() {
+  if (exec) cudaGraphExecDestroy(exec);
+  exec = nullptr;
+  nodes = 0;
+  key.clear();
+}
+
+void StepGraph::capture(cudaStream_t st, const std::vector<int64_t>& k, const std::function<void()>& step) {
+  if (exec && key == k) return;
+  reset();
+  cudaGraph_t g = nullptr;
+  const int64_t before = g_kernel_launches.load();
+  CT2_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+  try {
+    step();
+  } catch (...) {
+    cudaStreamEndCapture(st, &g);
+    if (g) cudaGraphDestroy(g);
+    throw;
+  }
+  CT2_CUDA_CHECK(cudaStreamEndCapture(st, &g));
+  g_kernel_launches.store(before);     // captured launches are counted when the graph is replayed
+  size_t n = 0;
+  cudaGraphGetNodes(g, nullptr, &n);
+  nodes = static_cast<int64_t>(n);
+  CT2_CUDA_CHECK(cudaGraphInstantiate(&exec, g, 0));
+  cudaGraphDestroy(g);
+  key = k;
+}
+
+void StepGraph::launch(cudaStream_t st) {
+  CT2_CUDA_CHECK(cudaGraphLaunch(exec, st));
+  count_launch(static_cast<int>(nodes));
+}
+
+int64_t eos_poll_interval() {
+  const char* env = std::getenv("CT2B200_EOS_POLL");
+  return std::max<int64_t>(1, env ? std::atoll(env) : 4);
+}
+
 // host-side conversion of a float-ish variable to the compute dtype
 std::vector<uint8_t> convert_to_dtype(const HostVariable& v, int dtype) {
   const int64_t n = v.size();
@@ -1064,7 +1104,6 @@ Generator::Generator(const std::string& model_dir, const ct2b200_generator_confi
 }
 
 Generator::~Generator() {
-  if (graph_) cudaGraphExecDestroy(graph_);
   if (host_pinned_) cudaFreeHost(host_pinned_);
   if (score_pinned_) cudaFreeHost(score_pinned_);
 }
@@ -1084,7 +1123,7 @@ void Generator::run_prefill(const int32_t* ids_d, int64_t batch, int64_t time,
   }
 }
 
-void Generator::launch_step(int64_t batch, int64_t, int) {
+void Generator::launch_step(int64_t batch) {
   LlamaDecoder& d = *decoder_;
   d.forward_step(ids_d_.as<int32_t>(), attn_lens_d_.as<int32_t>(), batch, d.logits_buffer());
   launch_sample_greedy(d.logits_buffer(), batch, d.config().vocab, step_d_.as<int32_t>(), end_ids_d_.as<int32_t>(),
@@ -1093,35 +1132,6 @@ void Generator::launch_step(int64_t batch, int64_t, int) {
                        sample_ws_.as<int32_t>() + d.max_batch() * 64, sample_ws_.as<float>() + d.max_batch() * 65,
                        want_scores_ ? scores_d_.as<float>() : nullptr, row_start_d_.as<int32_t>(), attn_lens_d_.as<int32_t>(),
                        finished_d_.as<int32_t>(), d.dtype(), d.stream());
-}
-
-void Generator::build_step_graph(int64_t batch, int64_t min_length, int num_end_ids) {
-  if (graph_ && graph_batch_ == batch && graph_scores_ == want_scores_) return;
-  if (graph_) {
-    cudaGraphExecDestroy(graph_);
-    graph_ = nullptr;
-  }
-  cudaStream_t st = decoder_->stream();
-  cudaGraph_t g = nullptr;
-  const int64_t before = g_kernel_launches.load();
-  CT2_CUDA_CHECK(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-  try {
-    launch_step(batch, min_length, num_end_ids);
-  } catch (...) {
-    cudaStreamEndCapture(st, &g);
-    if (g) cudaGraphDestroy(g);
-    throw;
-  }
-  CT2_CUDA_CHECK(cudaStreamEndCapture(st, &g));
-  g_kernel_launches.store(before);     // captured launches are counted when the graph is replayed
-  graph_nodes_ = 0;
-  size_t n = 0;
-  cudaGraphGetNodes(g, nullptr, &n);
-  graph_nodes_ = static_cast<int64_t>(n);
-  CT2_CUDA_CHECK(cudaGraphInstantiate(&graph_, g, 0));
-  cudaGraphDestroy(g);
-  graph_batch_ = batch;
-  graph_scores_ = want_scores_;
 }
 
 void Generator::generate(const GenerationRequest& r, int32_t* out_ids, int32_t* out_lens, float* out_scores) {
@@ -1184,7 +1194,7 @@ void Generator::generate(const GenerationRequest& r, int32_t* out_ids, int32_t* 
   launch_fill_i32(finished_d_.as<int32_t>(), B, 0, st);
 
   const bool use_graph = cfg_.use_cuda_graph != 0;
-  if (use_graph) build_step_graph(B, r.min_length, static_cast<int>(r.end_ids.size()));
+  if (use_graph) graph_.capture(st, {B, want_scores_}, [&] { launch_step(B); });
 
   // ---- GreedySearch::search host loop (decoding.cc:844-971) ----
   std::vector<std::vector<int32_t>> results(B);
@@ -1202,8 +1212,7 @@ void Generator::generate(const GenerationRequest& r, int32_t* out_ids, int32_t* 
   if (!r.end_ids.empty())
     for (int64_t b = 0; b < B; ++b)
       first_eos_step = std::min<int64_t>(first_eos_step, hstart[b] + std::max<int64_t>(0, r.min_length));
-  const char* poll_env = std::getenv("CT2B200_EOS_POLL");
-  const int64_t poll = std::max<int64_t>(1, poll_env ? std::atoll(poll_env) : 4);
+  const int64_t poll = eos_poll_interval();
   int32_t* hout = host_pinned_;     // reuse: [steps, B] sampled ids
   int64_t copied = 0;
   auto consume = [&](int64_t upto) {   // host bookkeeping for steps [copied, upto)
@@ -1240,11 +1249,10 @@ void Generator::generate(const GenerationRequest& r, int32_t* out_ids, int32_t* 
   };
   for (int64_t s = 0; s < total_steps && num_finished < B; ++s) {
     if (use_graph) {
-      CT2_CUDA_CHECK(cudaGraphLaunch(graph_, st));
-      count_launch(static_cast<int>(graph_nodes_));
+      graph_.launch(st);
     } else {
       pdl_fence_next_launch();
-      launch_step(B, r.min_length, static_cast<int>(r.end_ids.size()));
+      launch_step(B);
     }
     if (s + 1 == total_steps || (s >= first_eos_step && (s - first_eos_step) % poll == poll - 1)) consume(s + 1);
   }
@@ -1306,8 +1314,7 @@ std::vector<TranslationHypotheses> Generator::generate_beam(const GenerationRequ
   CT2_CUDA_CHECK(cudaMemcpyAsync(beam_->next_ids.ptr, start.data(), N * 4, cudaMemcpyHostToDevice, st));
   CT2_CUDA_CHECK(cudaStreamSynchronize(st));
 
-  const char* poll_env = std::getenv("CT2B200_EOS_POLL");
-  const int64_t poll = std::max<int64_t>(1, poll_env ? std::atoll(poll_env) : 4);
+  const int64_t poll = eos_poll_interval();
   const int64_t first_check = std::max<int64_t>(0, r.min_length);
   for (int64_t s = 0; s < L; ++s) {
     launch_fill_i32(lens_d_.as<int32_t>(), N, static_cast<int32_t>(fwd + s), st);
@@ -1461,14 +1468,12 @@ void Generator::bench_decode(int64_t batch, int64_t prompt_len, int64_t steps, i
   launch_fill_i32(attn_lens_d_.as<int32_t>(), batch, static_cast<int32_t>(fwd), st);
   launch_fill_i32(finished_d_.as<int32_t>(), batch, 0, st);
   const bool use_graph = cfg_.use_cuda_graph != 0;
-  if (use_graph) build_step_graph(batch, 0, 0);
+  if (use_graph) graph_.capture(st, {batch, want_scores_}, [&] { launch_step(batch); });
   auto step = [&]() {
-    if (use_graph) {
-      CT2_CUDA_CHECK(cudaGraphLaunch(graph_, st));
-      count_launch(static_cast<int>(graph_nodes_));
-    } else {
-      launch_step(batch, 0, 0);
-    }
+    if (use_graph)
+      graph_.launch(st);
+    else
+      launch_step(batch);
   };
   for (int64_t s = 0; s < warmup; ++s) step();
   CT2_CUDA_CHECK(cudaStreamSynchronize(st));

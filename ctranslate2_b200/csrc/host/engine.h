@@ -82,6 +82,25 @@ struct DenseWeights {
   int group_size = 128;
 };
 
+// A decoding step captured once as a CUDA graph and replayed.  `key` holds everything the capture bakes in (kernel arguments
+// are values): capture() with another key captures again.  Captured launches are counted when the graph is replayed, not
+// when it is captured.
+struct StepGraph {
+  cudaGraphExec_t exec = nullptr;
+  int64_t nodes = 0;
+  std::vector<int64_t> key;
+  StepGraph() = default;
+  StepGraph(const StepGraph&) = delete;
+  StepGraph& operator=(const StepGraph&) = delete;
+  ~StepGraph() { reset(); }
+  void reset();
+  void capture(cudaStream_t st, const std::vector<int64_t>& key, const std::function<void()>& step);   // unless `key` is held
+  void launch(cudaStream_t st);
+};
+
+// CT2B200_EOS_POLL: decoding steps between two looks of the host at the finished entries (default 4, at least 1)
+int64_t eos_poll_interval();
+
 class ModelFile;
 // Dense matrix of `prefix` converted on the GPU to what the compute type asks for (Model::set_compute_type); true = int8
 bool load_dense_matrix(const ModelFile& f, const std::string& prefix, int dtype, int weight_type, cudaStream_t st,
@@ -249,8 +268,7 @@ class Generator {
   // state of positions [t0, t0 + tc) is complete, before the next chunk overwrites it
   void run_prefill(const int32_t* ids_d, int64_t batch, int64_t time,
                    const std::function<void(int64_t t0, int64_t tc)>& after_chunk = nullptr);
-  void build_step_graph(int64_t batch, int64_t min_length, int num_end_ids);
-  void launch_step(int64_t batch, int64_t min_length, int num_end_ids);
+  void launch_step(int64_t batch);
 
   ct2b200_generator_config cfg_;
   std::mutex mu_;                          // generate / forward / bench_decode are serialised per generator
@@ -259,7 +277,6 @@ class Generator {
   DeviceBuffer ids_d_, lens_d_, step_d_, forced_d_, out_d_, end_ids_d_, prompt_d_, sample_ws_, scores_d_, row_start_d_;
   DeviceBuffer attn_lens_d_, finished_d_;    // per row: cache length the attention kernel sees (0 once finished), finished flag
   bool want_scores_ = false;               // the step (and its CUDA graph) also writes per-step log-probabilities
-  bool graph_scores_ = false;
   int32_t* host_pinned_ = nullptr;
   size_t host_pinned_elems_ = 0;
   std::unique_ptr<struct BeamSearchArena> beam_;   // created by the first beam search
@@ -268,10 +285,7 @@ class Generator {
   DeviceBuffer score_slab_, score_idx_d_, score_out_d_;
   int64_t score_slab_rows_ = 0;
   int32_t* score_pinned_ = nullptr;        // host staging of the row / target ids (pinned: the copies stay asynchronous)
-  cudaGraphExec_t graph_ = nullptr;
-  int64_t graph_nodes_ = 0;
-  int64_t graph_batch_ = -1, graph_min_len_ = -1;
-  int graph_num_end_ = -1;
+  StepGraph graph_;                        // key: {batch, want_scores_}
 };
 
 }  // namespace ct2b200

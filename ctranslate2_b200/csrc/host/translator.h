@@ -158,18 +158,38 @@ class Translator {
   bool post_norm(const NormWeights& n, void* x, int64_t rows, const DenseWeights* next);
   void run_encoder(int64_t batch, int64_t S);
   void run_encoder_layers(int64_t batch, int64_t S, const int32_t* lens_d);
-  void run_whisper_encoder(int64_t batch, int64_t frames);
+  // encoder positions of `frames` input frames; refuses a features shape the encoder cannot take
+  int64_t whisper_positions(int64_t batch, int64_t frames) const;
+  // the Whisper encoder on features_h [batch, n_mels, frames] f32 (host) -> memory_; src_lens_ = every position
+  void encode_audio(const float* features_h, int64_t batch, int64_t frames);
+  // memory_ [rows, d_model] -> memory_h f32 (host); synchronises
+  void copy_memory_to_host(int64_t rows, float* memory_h);
   void run_search(const BeamState& bs, int64_t S, int64_t first_check);
   void project_memory(int64_t batch, int64_t S);
+  // decoder embeddings of `rows` ids at positions 0 .. time - 1 (step_ptr null) or at *step_ptr (time 1) -> x_
+  void embed_decoder(const int32_t* ids_d, int64_t rows, int64_t time, const int32_t* step_ptr);
   // the decoder layer stack on `rows` rows of x_; `self_attention(layer)` fills ctx_ from qkv_, and each run of
   // `rows_per_entry` rows attends to one memory entry.  Returns whether xq_ / xs_ hold Quantize(x_).
   // `capture` (one entry per layer, count 0 = none): the cross-attention also saves the scores of those heads
   bool run_decoder_layers(int64_t rows, int rows_per_entry, int64_t S, const std::function<void(int)>& self_attention,
                           const std::vector<AttnCapture>* capture = nullptr);
+  // the teacher-forced pass of score / whisper_align / whisper_detect_language: `entries` sequences of T decoder inputs ids_d
+  // [entries * T] at positions 0 .. T - 1 with causal self-attention, each attending to its memory entry of S positions.
+  // Returns whether xq_ / xs_ hold Quantize(x_).
+  bool decode_teacher_forced(int64_t entries, int64_t T, int64_t S, const int32_t* ids_d,
+                             const std::vector<AttnCapture>* capture = nullptr);
+  // final norm + projection of n rows of x_ (rows_d [n]; null: the first n rows, at most one slab, with xq = what
+  // decode_teacher_forced returned) in slabs of score_slab_rows_ into score_logits_; reduce(logits, first, count, ld) runs on
+  // each slab's rows [first, first + count)
+  void project_rows(const int32_t* rows_d, int64_t n, bool xq,
+                    const std::function<void(const void*, int64_t, int64_t, int64_t)>& reduce);
   // the score slab, allocated on first use; returns the row stride of its logits
   int64_t ensure_score_slab();
+  // copies `ids` into score_ids_ (grown as needed); `ids` must stay alive until the copy is done
+  const int32_t* stage_ids(const std::vector<int32_t>& ids);
   void decoder_step(int64_t rows, int beam, int64_t batch, int64_t S);
-  void launch_or_capture_step(const BeamState& bs, int64_t S);
+  // one decoding step, captured as the graph of `key` (everything the capture bakes in) unless use_graph_ is off
+  void launch_or_capture_step(const BeamState& bs, int64_t S, const std::vector<int64_t>& key);
 
   std::mutex mu_;                // translate / score / encode / bench are serialised per translator
   Seq2SeqConfig mc_;
@@ -197,6 +217,7 @@ class Translator {
   DeviceBuffer features_, cols_, conv_out_, suppress_d_, forced_d_, no_speech_d_;   // Whisper
   int64_t cap_frames_ = 0;
   int64_t cap_fe_batch_ = 0, cap_fe_src_ = 0;                    // Whisper front-end buffers
+  std::vector<int32_t> audio_lens_h_;    // source of encode_audio's src_lens_ copy, alive until the call synchronises
   int32_t* host_pinned_ = nullptr;
   size_t host_pinned_elems_ = 0;
   // score: logits slab [score_slab_rows_, vocab (padded)], per pass: decoder input ids | scored rows | their target ids, scores
@@ -205,9 +226,7 @@ class Translator {
   // whisper_align: captured scores [entries, heads, T, S], standardised DTW rows [entries, heads, text + 1, S], DTW matrix
   DeviceBuffer align_scores_, align_norm_, align_matrix_, align_masks_;
 
-  cudaGraphExec_t graph_ = nullptr;
-  int64_t graph_nodes_ = 0;
-  std::vector<int64_t> graph_key_;
+  StepGraph graph_;
 };
 
 }  // namespace ct2b200
