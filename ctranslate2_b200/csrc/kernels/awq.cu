@@ -23,6 +23,7 @@
 #include "awq_common.cuh"
 #include "gemm_common.cuh"
 #include "kernels.h"
+#include "streamk.cuh"
 #include "tc_common.cuh"
 
 namespace ct2b200 {
@@ -120,12 +121,13 @@ constexpr int kPackedTile = kTileM * kBKh / 2;      // 4096 bytes of nibbles per
 
 struct AwqParams {
   int64_t n, m, k;
-  int tiles_a, kb_total, group;
+  int group;
+  sk::Schedule sched;
   const __half* sc[2];     // [n, k/group] scales (index 1: GLU "up" matrix)
   const __half* zr[2];
   FloatEpilogue fl;
   FloatGluEpilogue glu;
-  float* ws;               // partial-tile slots [ctas][2][NB][128*BN]
+  uint32_t* slots;         // partial-tile slots of the shared tiles [ctas][2][NB * 128 * BN]
   int32_t* counters;
 };
 
@@ -142,7 +144,7 @@ struct AwqSmem {
 
 // epilogue of one output channel over kCols batch rows; loads first, then arithmetic + stores
 template <int NB, int kCols>
-__device__ __forceinline__ void awq_chunk_epilogue(const AwqParams& p, const float (&acc)[NB][32], int64_t nrow, int64_t m0) {
+__device__ __forceinline__ void awq_chunk_epilogue(const AwqParams& p, const uint32_t (&acc)[NB][kCols], int64_t nrow, int64_t m0) {
   if (nrow >= p.n) return;
   const int64_t rows = min(static_cast<int64_t>(kCols), p.m - m0);
   if (rows <= 0) return;
@@ -151,8 +153,8 @@ __device__ __forceinline__ void awq_chunk_epilogue(const AwqParams& p, const flo
 #pragma unroll
     for (int j = 0; j < kCols; ++j) {
       if (j >= rows) break;
-      const float g = round_to<__half>(apply_act(round_to<__half>(acc[0][j]), p.glu.act));
-      h[(m0 + j) * p.glu.ldh + nrow] = __float2half_rn(g * round_to<__half>(acc[1][j]));
+      const float g = round_to<__half>(apply_act(round_to<__half>(__uint_as_float(acc[0][j])), p.glu.act));
+      h[(m0 + j) * p.glu.ldh + nrow] = __float2half_rn(g * round_to<__half>(__uint_as_float(acc[1][j])));
     }
   } else {
     const __half* bias = static_cast<const __half*>(p.fl.bias);
@@ -165,7 +167,7 @@ __device__ __forceinline__ void awq_chunk_epilogue(const AwqParams& p, const flo
 #pragma unroll
     for (int j = 0; j < kCols; ++j) {
       if (j >= rows) break;
-      float v = round_to<__half>(acc[0][j]);
+      float v = round_to<__half>(__uint_as_float(acc[0][j]));
       if (bias) v = round_to<__half>(v + b);
       if (p.fl.act >= 0) v = round_to<__half>(apply_act(v, p.fl.act));
       if (residual) v = v + res[j];
@@ -187,71 +189,34 @@ __global__ void __launch_bounds__(kAwqThreads, 1)
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(ring + kStages * S::kStage);
   uint64_t* empty_bar = full_bar + kStages;
   uint64_t* ready_bar = empty_bar + kStages;           // dequantized A tile of the stage is in place
-  __shared__ int s_last;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int64_t KB = p.kb_total;
-  const int64_t U = static_cast<int64_t>(p.tiles_a) * KB;
-  const int64_t P = gridDim.x;
-  const int64_t u_begin = blockIdx.x * U / P, u_end = (blockIdx.x + 1) * U / P;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < kStages; ++s) {
-      mbar_init(full_bar + s, 1);
-      mbar_init(empty_bar + s, 4);                     // one arrive per consumer warp
-      mbar_init(ready_bar + s, kDeqWarps);
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  __syncthreads();
-  griddep_launch();
+  int64_t u_begin, u_end;
+  p.sched.range(blockIdx.x, u_begin, u_end);
+  if (threadIdx.x == 0)
+    for (int s = 0; s < kStages; ++s) mbar_init(ready_bar + s, kDeqWarps);
+  ring_init<1>(full_bar, empty_bar, kStages);
 
   if (warp == kProducerWarp) {
     // ===== TMA producer: packed weight tile(s) + activation tile =====
     if (elect_one()) {
-      int it = 0;
-      int tile = static_cast<int>(u_begin / KB);
-      int kb = static_cast<int>(u_begin - tile * KB);
-      auto issue = [&](int s, int t_, int kb_, bool weights, bool acts) {
-        uint8_t* st = ring + s * S::kStage;
-        if (weights) {
-          tma_load_2d(st + S::kA, &tm_w, full_bar + s, kb_ * (kBKh / 2), t_ * kTileM, kEvictFirst);
-          if (NB == 2) tma_load_2d(st + S::kA + kPackedTile, &tm_w2, full_bar + s, kb_ * (kBKh / 2), t_ * kTileM, kEvictFirst);
-        }
-        if (acts) tma_load_2d(st + S::kA + S::kP, &tm_x, full_bar + s, kb_ * kBKh, 0, kEvictLast);
+      sk::Cursor wc(p.sched, u_begin), xc = wc;      // unit of the next weight / activation copy
+      auto weights = [&](int s, int) {
+        uint8_t* st = ring + s * S::kStage + S::kA;
+        tma_load_2d(st, &tm_w, full_bar + s, wc.kb * (kBKh / 2), wc.ta * kTileM, kEvictFirst);
+        if (NB == 2) tma_load_2d(st + kPackedTile, &tm_w2, full_bar + s, wc.kb * (kBKh / 2), wc.ta * kTileM, kEvictFirst);
+        wc.next(p.sched);
       };
-      // weights never depend on the previous kernel: fill the ring with them before griddepcontrol.wait
-      const int64_t prefill = min(static_cast<int64_t>(kStages), u_end - u_begin);
-      {
-        int t2 = tile, k2 = kb;
-        for (int64_t i = 0; i < prefill; ++i, ++k2) {
-          if (k2 == KB) { k2 = 0; ++t2; }
-          mbar_expect_tx(full_bar + i, S::kP + S::kX);
-          issue(static_cast<int>(i), t2, k2, true, false);
-        }
-      }
-      griddep_wait();
-      for (int64_t u = u_begin; u < u_end; ++u, ++it, ++kb) {
-        if (kb == KB) { kb = 0; ++tile; }
-        const int s = it % kStages;
-        const uint32_t ph = (it / kStages) & 1;
-        if (it < prefill) {
-          issue(s, tile, kb, false, true);
-        } else {
-          mbar_wait(empty_bar + s, ph ^ 1);
-          mbar_expect_tx(full_bar + s, S::kP + S::kX);
-          issue(s, tile, kb, true, true);
-        }
-      }
+      auto acts = [&](int s, int) {
+        tma_load_2d(ring + s * S::kStage + S::kA + S::kP, &tm_x, full_bar + s, xc.kb * kBKh, 0, kEvictLast);
+        xc.next(p.sched);
+      };
+      produce(full_bar, empty_bar, kStages, S::kP + S::kX, static_cast<int>(u_begin), static_cast<int>(u_end - u_begin), weights, acts);
     }
   } else if (warp > kProducerWarp) {
     // ===== dequantize warps: packed nibbles -> fp16 (q - z) * s into the swizzled wgmma A tile =====
     const int r = threadIdx.x - (kProducerWarp + 1) * 32;   // tile row owned by this thread
     const int64_t ng = p.k / p.group;
-    int it = 0;
-    int tile = static_cast<int>(u_begin / KB);
-    int kb = static_cast<int>(u_begin - tile * KB);
     // group scale / zero are fetched one group ahead (they change every group/64 K blocks), so the global-load
     // latency is off the per-block critical path
     int64_t cur_g = -1;
@@ -265,8 +230,9 @@ __global__ void __launch_bounds__(kAwqThreads, 1)
         sc[w] = ok ? p.sc[w][row * ng + g] : __float2half(0.f);
       }
     };
-    for (int64_t u = u_begin; u < u_end; ++u, ++it, ++kb) {
-      if (kb == KB) { kb = 0; ++tile; }
+    sk::Cursor cur(p.sched, u_begin);
+    for (int it = 0; it < u_end - u_begin; ++it, cur.next(p.sched)) {
+      const int tile = cur.ta, kb = cur.kb;
       const int s = it % kStages;
       const uint32_t ph = (it / kStages) & 1;
       const int64_t row = static_cast<int64_t>(tile) * kTileM + r;
@@ -306,96 +272,37 @@ __global__ void __launch_bounds__(kAwqThreads, 1)
   } else {
     // ===== consumer warpgroup: wgmma over a segment's K blocks, then its epilogue =====
     griddep_wait();                                     // bias / residual may come from the previous kernel
-    const int q = warp & 3;
-    const int et = threadIdx.x;
+    constexpr int kC = BN < 32 ? BN : 32;               // columns per chunk
+    const int rloc = threadIdx.x;                       // output channel of the tile owned by this thread
     int it = 0;
-    const int64_t slot_elems = static_cast<int64_t>(NB) * kTileM * BN;
-    for (int64_t u = u_begin; u < u_end;) {
-      const int64_t tile = u / KB;
-      const int kb0 = static_cast<int>(u - tile * KB);
-      const int kb1 = static_cast<int>(min(KB, static_cast<int64_t>(kb0) + (u_end - u)));
-      u += kb1 - kb0;
-      const int64_t a0 = tile * kTileM;
-      const bool direct = kb0 == 0 && kb1 == KB;
-      float* my_slot = p.ws + (static_cast<int64_t>(blockIdx.x) * 2 + (kb0 > 0 ? 0 : 1)) * slot_elems;
-      {
-        Acc<BN> acc[NB];
+    auto mma = [&](int kb0, int kb1) {
+      Acc<BN> acc[NB];
 #pragma unroll 1
-        for (int kb = kb0; kb < kb1; ++kb, ++it) {
-          const int s = it % kStages;
-          const uint32_t ph = (it / kStages) & 1;
-          mbar_wait(full_bar + s, ph);                  // activations landed
-          mbar_wait(ready_bar + s, ph);                 // weights dequantized
-          const uint32_t sa = smem_u32(ring + s * S::kStage);
-          wgmma_fence();
+      for (int kb = kb0; kb < kb1; ++kb, ++it) {
+        const int s = it % kStages;
+        const uint32_t ph = (it / kStages) & 1;
+        mbar_wait(full_bar + s, ph);                    // activations landed
+        mbar_wait(ready_bar + s, ph);                   // weights dequantized
+        const uint32_t sa = smem_u32(ring + s * S::kStage);
+        wgmma_fence();
 #pragma unroll
-          for (int w = 0; w < NB; ++w) mma_block<1, BN>(acc[w], sa + w * kTileM * kSwizzleBytes, sa + S::kA + S::kP, kb == kb0);
-          wgmma_commit();
-          wgmma_wait();
-          if (lane == 0) mbar_arrive(empty_bar + s);
-        }
-        epi_bar_sync();                                 // the previous segment's rows have been read out of accs
-#pragma unroll
-        for (int w = 0; w < NB; ++w) acc_store<BN>(acc[w], accs + w * BN * kAccPitch);
-        epi_bar_sync();
+        for (int w = 0; w < NB; ++w) mma_block<1, BN>(acc[w], sa + w * kTileM * kSwizzleBytes, sa + S::kA + S::kP, kb == kb0);
+        wgmma_commit();
+        wgmma_wait();
+        if (lane == 0) mbar_arrive(empty_bar + s);
       }
-      const int rloc = q * 32 + lane;
-      const int64_t nrow = a0 + rloc;                   // output channel owned by this thread
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t rr[NB][32];
+      epi_bar_sync();                                   // the previous segment's rows have been read out of accs
 #pragma unroll
-        constexpr int kCols = (BN % 32 == 0) ? 32 : 16;
-#pragma unroll
-        for (int w = 0; w < NB; ++w)
-#pragma unroll
-          for (int j = 0; j < kCols; ++j) rr[w][j] = accs[((w * BN + c0) + j) * kAccPitch + rloc];
-        if (direct) {
-          float acc[NB][32];
-#pragma unroll
-          for (int w = 0; w < NB; ++w)
-#pragma unroll
-            for (int j = 0; j < kCols; ++j) acc[w][j] = __uint_as_float(rr[w][j]);
-          awq_chunk_epilogue<NB, kCols>(p, acc, nrow, c0);
-        } else {
-#pragma unroll
-          for (int j = 0; j < kCols; ++j)
-#pragma unroll
-            for (int w = 0; w < NB; ++w)     // slot layout [w][m][128 channels]: coalesced across the warp
-              my_slot[(static_cast<int64_t>(w) * BN + c0 + j) * kTileM + rloc] = __uint_as_float(rr[w][j]);
-        }
-      }
-      if (direct) continue;
-      __threadfence();
+      for (int w = 0; w < NB; ++w) acc_store<BN>(acc[w], accs + w * BN * kAccPitch);
       epi_bar_sync();
-      const int c_lo = cta_of_unit(tile * KB, U, P), c_hi = cta_of_unit((tile + 1) * KB - 1, U, P);
-      if (et == 0) s_last = atomicAdd(p.counters + tile, 1) == (c_hi - c_lo);
-      epi_bar_sync();
-      if (s_last) {
-        __threadfence();
-        constexpr int kColsF = (BN % 32 == 0) ? 32 : 16;
-#pragma unroll 1
-        for (int c0 = 0; c0 < BN; c0 += kColsF) {
-          float acc[NB][32];
-#pragma unroll
-          for (int w = 0; w < NB; ++w)
-#pragma unroll
-            for (int j = 0; j < kColsF; ++j) acc[w][j] = 0.f;
-          for (int c = c_lo; c <= c_hi; ++c) {           // fixed order => deterministic sum
-            const float* sl = p.ws + (static_cast<int64_t>(c) * 2 + (c == c_lo ? 1 : 0)) * slot_elems;
-#pragma unroll
-            for (int w = 0; w < NB; ++w)
-#pragma unroll
-              for (int j = 0; j < kColsF; ++j) acc[w][j] += __ldcg(sl + (static_cast<int64_t>(w) * BN + c0 + j) * kTileM + et);
-          }
-          awq_chunk_epilogue<NB, kColsF>(p, acc, a0 + et, c0);
-        }
-        if (et == 0) p.counters[tile] = 0;
-      }
-      epi_bar_sync();
-    }
+    };
+    struct NoInputs {};
+    auto load = [](NoInputs&, int64_t, int64_t) {};
+    auto finish = [&](const NoInputs&, const uint32_t (&r)[NB][kC], int64_t a0, int64_t m0) {
+      awq_chunk_epilogue<NB, kC>(p, r, a0 + rloc, m0);
+    };
+    sk::consume<NB, BN, kC, false, NoInputs>(p.sched, blockIdx.x, u_begin, u_end, p.m, accs, p.slots, p.counters, mma, load, finish);
   }
-
 }
 
 CUtensorMap make_packed_map(const void* wp, int64_t n, int64_t k) {
@@ -421,18 +328,14 @@ void launch_awq(const void* x, const AwqNative& w, const AwqNative* w2, int64_t 
   const CUtensorMap tmw = make_packed_map(w.wp, w.n, w.k);
   const CUtensorMap tmw2 = make_packed_map(w2 ? w2->wp : w.wp, w.n, w.k);
   p.n = w.n; p.m = m; p.k = w.k; p.group = w.group;
-  p.tiles_a = div_up(w.n, kTileM);
-  p.kb_total = div_up(w.k, kBKh);
   p.sc[0] = static_cast<const __half*>(w.sc); p.zr[0] = static_cast<const __half*>(w.zr);
   p.sc[1] = static_cast<const __half*>(w2 ? w2->sc : w.sc); p.zr[1] = static_cast<const __half*>(w2 ? w2->zr : w.zr);
   SplitKWorkspace& wsp = SplitKWorkspace::get(st);
-  const int64_t units = static_cast<int64_t>(p.tiles_a) * p.kb_total;
-  const int64_t ctas = std::min<int64_t>(wsp.sm_count, units);
-  CT2_REQUIRE(static_cast<size_t>(ctas) * 2 * NB * kTileM * BN <= wsp.accum_elems && static_cast<size_t>(p.tiles_a) <= wsp.num_counters,
-              "awq: scratch too small");
-  p.ws = reinterpret_cast<float*>(wsp.accum2);
+  p.sched = sk::stream_k(div_up(w.n, kTileM), 1, div_up(w.k, kBKh), wsp.sm_count);
+  CT2_REQUIRE(sk::slots_fit(p.sched, NB * kTileM * BN, wsp), "awq: scratch too small");
+  p.slots = reinterpret_cast<uint32_t*>(wsp.accum2);
   p.counters = wsp.counters;
-  launch_pdl(kernel, dim3(static_cast<unsigned>(ctas)), dim3(kAwqThreads), S::kBytes, st, tmx, tmw, tmw2, p);
+  launch_pdl(kernel, dim3(static_cast<unsigned>(p.sched.ctas)), dim3(kAwqThreads), S::kBytes, st, tmx, tmw, tmw2, p);
   check_launch();
 }
 

@@ -113,7 +113,7 @@ __global__ void __launch_bounds__(kTcThreads, 2)
 template <int BN, int NB>
 int stages_for(int cs, int nkb) {
   using S = DecSmem<BN, NB>;
-  const size_t cap = static_cast<size_t>(std::max(48, std::min(200, env_int("CT2B200_GEMM_SMEM_KB", 200)))) * 1024;
+  constexpr size_t cap = 200 * 1024;
   int st = static_cast<int>((cap - S::kAcc - S::kCtrl - red_bytes(cs, NB, BN) - 1024) / S::kStage);
   st = std::max(2, std::min(st, kMaxStages));
   return std::max(2, std::min(st, std::max(nkb, 2)));

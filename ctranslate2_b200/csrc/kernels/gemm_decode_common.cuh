@@ -1,6 +1,6 @@
 // gemm_decode_common.cuh — pieces shared by the decode (weight-streaming) wgmma kernels: gemm_decode.cu (INT8 / f16
-// weights) and awq_decode.cu (AWQ-INT4 weights): the operand ring, the split-K
-// cluster exchange with its fused epilogue of one output channel, and the planner / launch helpers.
+// weights) and awq_decode.cu (AWQ-INT4 weights): the split-K cluster exchange with its fused epilogue of one output
+// channel, and the planner / launch helpers.
 #pragma once
 
 #include <algorithm>
@@ -41,9 +41,6 @@ struct DecParams {
   int act;
   int64_t ldy;
 };
-
-__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
-__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 
 // One thread finishes NC output elements of its channel `arow`: batch rows col0, col0 + cstep, ...
 // r[w][j] = raw accumulators (int32 or fp32 bits).
@@ -95,48 +92,6 @@ constexpr int owned_per_chunk(int cs) { return (16 + cs - 1) / cs; }
 // exchange buffer [cs source ranks][nb weights][(bn / 16) chunks x owned columns][128 channels] of 32-bit partials
 constexpr size_t red_bytes(int cs, int nb, int bn) {
   return cs > 1 ? static_cast<size_t>(cs) * nb * (bn / 16) * owned_per_chunk(cs) * kTileM * 4 : 0;
-}
-
-// mbarriers of the operand ring; then the next kernel may be scheduled, and phase 1 of the cluster barrier is signalled
-// (this CTA is alive: peers may write its shared memory once they have waited for the phase)
-template <int CS>
-__device__ __forceinline__ void ring_init(uint64_t* full_bar, uint64_t* free_bar, int nstages) {
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < nstages; ++s) {
-      mbar_init(full_bar + s, 1);
-      mbar_init(free_bar + s, 4);                    // one arrive per consumer warp
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  }
-  __syncthreads();
-  griddep_launch();
-  if (CS > 1) cluster_arrive();
-}
-
-// Producer schedule of one elected lane over blocks [lo, lo + n): weights(slot, block) and acts(slot, block) issue the
-// copies of one ring slot (tx_bytes in all).  The weights never depend on the previous kernel, so the first ring fill is
-// issued BEFORE the dependency wait and overlaps the predecessor's tail.
-template <typename W, typename A>
-__device__ __forceinline__ void produce(uint64_t* full_bar, uint64_t* free_bar, int nstages, uint32_t tx_bytes, int lo, int n,
-                                        const W& weights, const A& acts) {
-  const int pre = min(nstages, n);
-#pragma unroll 1
-  for (int i = 0; i < pre; ++i) {
-    mbar_expect_tx(full_bar + i, tx_bytes);
-    weights(i, lo + i);
-  }
-  griddep_wait();
-#pragma unroll 1
-  for (int i = 0; i < pre; ++i) acts(i, lo + i);
-#pragma unroll 1
-  for (int it = pre; it < n; ++it) {
-    const int s = it % nstages;
-    mbar_wait(free_bar + s, ((it / nstages) & 1) ^ 1);
-    mbar_expect_tx(full_bar + s, tx_bytes);
-    weights(s, lo + it);
-    acts(s, lo + it);
-  }
 }
 
 // Epilogue with thread = output channel.  EVERY warp of the CTA calls it as the last thing it does: the consumer warps

@@ -1,6 +1,6 @@
 // tc_common.cuh — inline-PTX wrappers shared by the wgmma kernels (gemm_tc.cu, gemm_decode.cu, gemm_prefill.cu, awq.cu,
-// awq_decode.cu): mbarrier, TMA (cp.async.bulk.tensor), wgmma with its shared-memory descriptors, and the hand-over of
-// the register accumulators to the row-per-thread epilogues.
+// awq_decode.cu): mbarrier, TMA (cp.async.bulk.tensor), the operand ring (barrier set-up and producer schedule), wgmma with
+// its shared-memory descriptors, and the hand-over of the register accumulators to the row-per-thread epilogues.
 // Bit layouts follow cute::GmmaDescriptor (CUTLASS, cute/arch/mma_sm90_desc.hpp).
 #pragma once
 
@@ -185,10 +185,49 @@ __device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 128;"
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
   asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 
-// index of the CTA whose unit range [c*U/P, (c+1)*U/P) contains unit u
-__device__ __forceinline__ int cta_of_unit(int64_t u, int64_t U, int64_t P) {
-  return static_cast<int>(((u + 1) * P + U - 1) / U - 1);
+// mbarriers of the operand ring; then the next kernel may be scheduled, and phase 1 of the cluster barrier is signalled
+// (this CTA is alive: peers may write its shared memory once they have waited for the phase)
+template <int CS>
+__device__ __forceinline__ void ring_init(uint64_t* full_bar, uint64_t* free_bar, int nstages) {
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < nstages; ++s) {
+      mbar_init(full_bar + s, 1);
+      mbar_init(free_bar + s, 4);                    // one arrive per consumer warp
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  }
+  __syncthreads();
+  griddep_launch();
+  if (CS > 1) cluster_arrive();
+}
+
+// Producer schedule of one elected lane over blocks [lo, lo + n): weights(slot, block) and acts(slot, block) issue the
+// copies of one ring slot (tx_bytes in all).  The weights never depend on the previous kernel, so the first ring fill is
+// issued BEFORE the dependency wait and overlaps the predecessor's tail.
+template <typename W, typename A>
+__device__ __forceinline__ void produce(uint64_t* full_bar, uint64_t* free_bar, int nstages, uint32_t tx_bytes, int lo, int n,
+                                        const W& weights, const A& acts) {
+  const int pre = min(nstages, n);
+#pragma unroll 1
+  for (int i = 0; i < pre; ++i) {
+    mbar_expect_tx(full_bar + i, tx_bytes);
+    weights(i, lo + i);
+  }
+  griddep_wait();
+#pragma unroll 1
+  for (int i = 0; i < pre; ++i) acts(i, lo + i);
+#pragma unroll 1
+  for (int it = pre; it < n; ++it) {
+    const int s = it % nstages;
+    mbar_wait(free_bar + s, ((it / nstages) & 1) ^ 1);
+    mbar_expect_tx(full_bar + s, tx_bytes);
+    weights(s, lo + it);
+    acts(s, lo + it);
+  }
 }
 
 
