@@ -55,3 +55,9 @@ class GeneratorConfig(ctypes.Structure):
 
 def kernel_launch_count() -> int:
     return int(lib().ct2b200_kernel_launch_count())
+
+
+def set_random_seed(seed: int):
+    """ctranslate2.set_random_seed: the process-wide seed of random sampling.  It also restarts the sampling-call counter, so
+    the same sequence of sampled calls after the same seed gives the same results."""
+    check(lib().ct2b200_set_random_seed(ctypes.c_uint32(int(seed) & 0xFFFFFFFF)))

@@ -13,6 +13,7 @@
 #include "host/translator.h"
 #include "kernels/beam_decide.h"
 #include "kernels/kernels.h"
+#include "kernels/philox.h"
 
 using namespace ct2b200;
 
@@ -229,6 +230,26 @@ CT2B200_API int ct2b200_topk(const void* x, int64_t rows, int64_t cols, int k, v
     require_device();
     CT2_REQUIRE(k >= 1 && k <= 64 && k <= cols, "topk: k must be in [1, min(64, cols)]");
     launch_topk(x, rows, cols, k, values, indices, dtype, S(stream));
+  });
+}
+
+CT2B200_API int ct2b200_random_sample(const void* x, int64_t rows, int64_t cols, int k, float temperature, uint32_t seed,
+                                      uint32_t counter, uint32_t step, int32_t* ids, float* logp, int dtype, void* stream) {
+  return guarded([&] {
+    require_device();
+    launch_random_sample(x, rows, cols, cols, k, temperature, seed, counter, step, ids, logp, dtype, S(stream));
+  });
+}
+
+CT2B200_API int ct2b200_set_random_seed(uint32_t seed) {
+  return guarded([&] { set_random_seed(seed); });
+}
+
+CT2B200_API int ct2b200_philox4x32_host(const uint32_t* counter, const uint32_t* key, uint32_t* out) {
+  return guarded([&] {
+    CT2_REQUIRE(counter && key && out, "philox4x32_host: null argument");
+    const Philox4 r = philox4x32_10(Philox4{{counter[0], counter[1], counter[2], counter[3]}}, key[0], key[1]);
+    for (int i = 0; i < 4; ++i) out[i] = r.v[i];
   });
 }
 
@@ -731,12 +752,13 @@ CT2B200_API int ct2b200_whisper_encode(ct2b200_translator* t, const float* featu
   });
 }
 
-CT2B200_API int ct2b200_whisper_generate(ct2b200_translator* t, const float* features, int64_t batch, int64_t frames,
-                             const int32_t* prompts, int64_t prompt_len, int beam_size, float patience, float length_penalty,
-                             int64_t max_length, int num_hypotheses, const int32_t* suppress_ids, int num_suppress,
-                             const int32_t* suppress_begin, int num_begin, int32_t sot_id, int32_t eot_id, int32_t no_speech_id,
-                             int32_t no_timestamps_id, int max_initial_timestamp_index, int32_t* out_ids, int32_t* out_lens,
-                             float* out_scores, float* no_speech) {
+namespace {
+int whisper_generate(ct2b200_translator* t, const float* features, int64_t batch, int64_t frames, const int32_t* prompts,
+                     int64_t prompt_len, int beam_size, float patience, float length_penalty, int64_t max_length, int num_hypotheses,
+                     const int32_t* suppress_ids, int num_suppress, const int32_t* suppress_begin, int num_begin, int32_t sot_id,
+                     int32_t eot_id, int32_t no_speech_id, int32_t no_timestamps_id, int max_initial_timestamp_index,
+                     int sampling_topk, float sampling_temperature, int32_t* out_ids, int32_t* out_lens, float* out_scores,
+                     float* no_speech) {
   return guarded([&] {
     CT2_REQUIRE(t && features && prompts && out_ids && out_lens && out_scores, "whisper_generate: null argument");
     WhisperRequest r;
@@ -757,8 +779,36 @@ CT2B200_API int ct2b200_whisper_generate(ct2b200_translator* t, const float* fea
     r.no_speech_id = no_speech_id;
     r.no_timestamps_id = no_timestamps_id;
     r.max_initial_timestamp_index = max_initial_timestamp_index;
+    r.sampling_topk = sampling_topk;
+    r.sampling_temperature = sampling_temperature;
     copy_hypotheses(t->impl->whisper_generate(r, no_speech), batch, num_hypotheses, max_length, out_ids, out_lens, out_scores);
   });
+}
+}  // namespace
+
+CT2B200_API int ct2b200_whisper_generate(ct2b200_translator* t, const float* features, int64_t batch, int64_t frames,
+                             const int32_t* prompts, int64_t prompt_len, int beam_size, float patience, float length_penalty,
+                             int64_t max_length, int num_hypotheses, const int32_t* suppress_ids, int num_suppress,
+                             const int32_t* suppress_begin, int num_begin, int32_t sot_id, int32_t eot_id, int32_t no_speech_id,
+                             int32_t no_timestamps_id, int max_initial_timestamp_index, int32_t* out_ids, int32_t* out_lens,
+                             float* out_scores, float* no_speech) {
+  return whisper_generate(t, features, batch, frames, prompts, prompt_len, beam_size, patience, length_penalty, max_length,
+                          num_hypotheses, suppress_ids, num_suppress, suppress_begin, num_begin, sot_id, eot_id, no_speech_id,
+                          no_timestamps_id, max_initial_timestamp_index, 1, 1.f, out_ids, out_lens, out_scores, no_speech);
+}
+
+CT2B200_API int ct2b200_whisper_generate_sampling(ct2b200_translator* t, const float* features, int64_t batch, int64_t frames,
+                                                  const int32_t* prompts, int64_t prompt_len, int beam_size, float patience,
+                                                  float length_penalty, int64_t max_length, int num_hypotheses,
+                                                  const int32_t* suppress_ids, int num_suppress, const int32_t* suppress_begin,
+                                                  int num_begin, int32_t sot_id, int32_t eot_id, int32_t no_speech_id,
+                                                  int32_t no_timestamps_id, int max_initial_timestamp_index, int sampling_topk,
+                                                  float sampling_temperature, int32_t* out_ids, int32_t* out_lens,
+                                                  float* out_scores, float* no_speech) {
+  return whisper_generate(t, features, batch, frames, prompts, prompt_len, beam_size, patience, length_penalty, max_length,
+                          num_hypotheses, suppress_ids, num_suppress, suppress_begin, num_begin, sot_id, eot_id, no_speech_id,
+                          no_timestamps_id, max_initial_timestamp_index, sampling_topk, sampling_temperature, out_ids, out_lens,
+                          out_scores, no_speech);
 }
 
 CT2B200_API int ct2b200_whisper_align(ct2b200_translator* t, const float* features, int64_t batch, int64_t frames,

@@ -3,13 +3,17 @@
 
 #include <algorithm>
 #include <cmath>
+#include <cstring>
+#include <mutex>
 #include <numeric>
+#include <random>
 
 namespace ct2b200 {
 
 BeamSearchArena::BeamSearchArena() {
   end_ids.alloc(64 * sizeof(int32_t));
   counters.alloc(64);
+  rng.alloc(2 * sizeof(uint32_t));
   CT2_CUDA_CHECK(cudaMemset(counters.ptr, 0, 64));
   CT2_CUDA_CHECK(cudaDeviceSynchronize());   // legacy-stream memset vs the engine's non-blocking stream
 }
@@ -39,6 +43,10 @@ bool BeamSearchArena::ensure(int64_t batch, int beam, int64_t steps, size_t es) 
   hyp_tokens.alloc(B * maxh * L * 4);
   hyp_len.alloc(B * maxh * 4);
   hyp_score.alloc(B * maxh * 4);
+  sample_ids.alloc(N * 4);
+  sample_logp.alloc(N * 4);
+  row_score.alloc(N * 4);
+  row_done.alloc(N * 4);
   const size_t need = static_cast<size_t>(B) * maxh * (L + 2) + B + 64;
   if (need > host_elems) {
     if (host) cudaFreeHost(host);
@@ -101,6 +109,29 @@ void BeamSearchArena::step(void* logits, const BeamState& bs, int dtype, cudaStr
   launch_beam_update(bs, cand_scores.ptr, cand_ids.as<int32_t>(), cum.ptr, false, dtype, st);
 }
 
+void BeamSearchArena::reset_sampling(BeamState& bs, int topk, float temperature, cudaStream_t st) {
+  bs.sample_topk = topk;
+  bs.sample_temperature = temperature;
+  bs.rng = rng.as<uint32_t>();
+  bs.sample_ids = sample_ids.as<int32_t>();
+  bs.sample_logp = sample_logp.as<float>();
+  bs.row_score = row_score.as<float>();
+  bs.row_done = row_done.as<int32_t>();
+  const int64_t N = static_cast<int64_t>(bs.batch) * bs.beam;
+  CT2_CUDA_CHECK(cudaMemsetAsync(row_score.ptr, 0, N * 4, st));
+  CT2_CUDA_CHECK(cudaMemsetAsync(row_done.ptr, 0, N * 4, st));
+  const SamplingCall c = next_sampling_call();
+  int32_t words[2];
+  std::memcpy(words, &c, sizeof(words));
+  launch_fill_i32(rng.as<int32_t>(), 1, words[0], st);
+  launch_fill_i32(rng.as<int32_t>() + 1, 1, words[1], st);
+}
+
+void BeamSearchArena::sample_step(void* logits, const BeamState& bs, int dtype, cudaStream_t st) {
+  launch_beam_sample(logits, bs, dtype, st);
+  launch_beam_sample_update(bs, st);
+}
+
 // finalize_result (decoding.cc:189-254): normalise by length^penalty, sort (stable: equal scores keep registration order), keep
 // num_hypotheses, strip `strip_ids` from the tail
 std::vector<TranslationHypotheses> BeamSearchArena::collect(const BeamState& bs, float length_penalty, int num_hypotheses,
@@ -136,6 +167,27 @@ std::vector<TranslationHypotheses> BeamSearchArena::collect(const BeamState& bs,
     }
   }
   return out;
+}
+
+namespace {
+std::mutex g_rng_mu;
+bool g_rng_seeded = false;
+SamplingCall g_rng{0, 0};
+}  // namespace
+
+void set_random_seed(uint32_t seed) {
+  std::lock_guard<std::mutex> lock(g_rng_mu);
+  g_rng = SamplingCall{seed, 0};
+  g_rng_seeded = true;
+}
+
+SamplingCall next_sampling_call() {
+  std::lock_guard<std::mutex> lock(g_rng_mu);
+  if (!g_rng_seeded) {
+    g_rng = SamplingCall{std::random_device{}(), 0};
+    g_rng_seeded = true;
+  }
+  return SamplingCall{g_rng.seed, g_rng.call++};
 }
 
 }  // namespace ct2b200

@@ -20,6 +20,7 @@ struct BeamSearchArena {
   int cap_beam = 0;
   DeviceBuffer cum, cand_scores, cand_ids, next_ids, end_ids, counters, finished, top_done, num_hyp, alive, anc, parent;
   DeviceBuffer hyp_tokens, hyp_len, hyp_score;
+  DeviceBuffer rng, sample_ids, sample_logp, row_score, row_done;   // sampled search
   int32_t* host = nullptr;                // pinned staging of the results
   size_t host_elems = 0;
 
@@ -38,8 +39,21 @@ struct BeamSearchArena {
   // one search step over logits [batch * beam, vocab] T (modified in place): log-probabilities + cumulative scores,
   // TopK of 2 * beam candidates per entry, bookkeeping; next_ids / cum / parent / histories are updated on the device
   void step(void* logits, const BeamState& bs, int dtype, cudaStream_t st);
+  // sampled search (GreedySearch with a RandomSampler): turns bs into a sampled state and clears the row scores; the rows of
+  // this call draw from (seed, call) of next_sampling_call()
+  void reset_sampling(BeamState& bs, int topk, float temperature, cudaStream_t st);
+  // one sampled step over logits [batch * beam, vocab] T (modified in place)
+  void sample_step(void* logits, const BeamState& bs, int dtype, cudaStream_t st);
   std::vector<TranslationHypotheses> collect(const BeamState& bs, float length_penalty, int num_hypotheses,
                                              const std::vector<int32_t>& strip_ids, cudaStream_t st);
 };
+
+// The process-wide random state of sampling (set_random_seed, src/random.cc): a seed, drawn once from std::random_device
+// unless set, and the index of the next sampling call, which every sampled search advances and set_random_seed resets.
+void set_random_seed(uint32_t seed);
+struct SamplingCall {
+  uint32_t seed, call;
+};
+SamplingCall next_sampling_call();
 
 }  // namespace ct2b200

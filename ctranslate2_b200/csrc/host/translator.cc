@@ -496,7 +496,10 @@ void Translator::launch_or_capture_step(const BeamState& bs, int64_t S, const st
   const int64_t rows = static_cast<int64_t>(bs.batch) * bs.beam;
   auto step = [&] {
     decoder_step(rows, bs.beam, bs.batch, S);
-    beam_.step(logits_.ptr, bs, dtype_, stream_);
+    if (bs.sample_topk >= 0)
+      beam_.sample_step(logits_.ptr, bs, dtype_, stream_);
+    else
+      beam_.step(logits_.ptr, bs, dtype_, stream_);
   };
   if (!use_graph_) {
     step();
@@ -512,9 +515,12 @@ void Translator::launch_or_capture_step(const BeamState& bs, int64_t S, const st
 // the decoding loop: one captured step per position; the host only polls the "finished entries" counter
 void Translator::run_search(const BeamState& bs, int64_t S, int64_t first_check) {
   // everything the captured step bakes in (kernel arguments are values)
+  uint32_t temperature_bits;
+  std::memcpy(&temperature_bits, &bs.sample_temperature, 4);
   std::vector<int64_t> key = {bs.batch, bs.beam, S, bs.vocab_ld, bs.stride, bs.max_steps, bs.min_length, bs.max_hyp, bs.max_candidates,
                               bs.num_hypotheses, bs.early_exit, bs.num_end, bs.start_step, bs.include_eos, bs.num_disable,
-                              bs.num_begin, bs.ts_begin, bs.ts_end, bs.ts_eot, bs.ts_no_timestamps, bs.ts_max_initial};
+                              bs.num_begin, bs.ts_begin, bs.ts_end, bs.ts_eot, bs.ts_no_timestamps, bs.ts_max_initial,
+                              bs.sample_topk, temperature_bits};
   const int64_t poll = eos_poll_interval();
   int32_t* hfin = beam_.host;
   for (int64_t s = 0; s < bs.max_steps; ++s) {
@@ -810,9 +816,15 @@ std::vector<TranslationHypotheses> Translator::whisper_generate(const WhisperReq
   CT2_REQUIRE(mc_.whisper, "whisper_generate needs a Whisper model");
   const int64_t B = r.batch, P = r.prompt_len, frames = r.frames;
   const int64_t S = whisper_positions(B, frames);
-  const int beam = r.beam_size;
-  CT2_REQUIRE(beam >= 1 && beam <= 32, "beam_size must be in [1, 32]");
-  CT2_REQUIRE(r.num_hypotheses >= 1 && r.num_hypotheses <= beam, "num_hypotheses must be in [1, beam_size]");
+  CT2_REQUIRE(r.beam_size >= 1 && r.beam_size <= 32, "beam_size must be in [1, 32]");
+  CT2_REQUIRE(r.sampling_topk >= 0 && r.sampling_temperature >= 0.f, "sampling_topk and sampling_temperature must be >= 0");
+  const bool sampling = r.sampling_topk != 1 && r.sampling_temperature != 0.f;     // decoding.cc:1067-1074
+  CT2_REQUIRE(!sampling || r.sampling_topk <= mc_.tgt_vocab, "sampling_topk is greater than the vocabulary size");
+  CT2_REQUIRE(!sampling || r.beam_size == 1, "random sampling with beam_size > 1 (sampled beam search) is not supported");
+  // a sampled call decodes num_hypotheses independent rows per entry, laid out like the rows of a beam
+  const int beam = sampling ? r.num_hypotheses : r.beam_size;
+  CT2_REQUIRE(r.num_hypotheses >= 1 && r.num_hypotheses <= (sampling ? 32 : r.beam_size),
+              sampling ? "num_hypotheses must be in [1, 32] when sampling" : "num_hypotheses must be in [1, beam_size]");
   CT2_REQUIRE(r.patience > 0.f && r.patience <= 2.f, "patience must be in (0, 2]");
   CT2_REQUIRE(r.suppress_ids.size() + r.suppress_ids_begin.size() <= 4096, "too many suppressed tokens");
   // check_prompts (whisper.cc:168-197): <|startoftranscript|> at the same position in every prompt and the same number of
@@ -878,6 +890,7 @@ std::vector<TranslationHypotheses> Translator::whisper_generate(const WhisperReq
     bs.ts_max_initial = bs.ts_begin + r.max_initial_timestamp_index;
   }
   beam_.reset(bs, r.prompts[0], dtype_, stream_);
+  if (sampling) beam_.reset_sampling(bs, r.sampling_topk, r.sampling_temperature, stream_);
   CT2_CUDA_CHECK(cudaMemcpyAsync(beam_.next_ids.ptr, forced_d_.ptr, N * 4, cudaMemcpyDeviceToDevice, stream_));
   no_speech_d_.alloc(B * 4);
   for (int64_t t = 0; t < start_step; ++t) {

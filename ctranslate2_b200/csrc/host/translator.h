@@ -85,6 +85,10 @@ struct WhisperRequest {
   int32_t sot_id = 0, eot_id = 0, no_speech_id = -1, no_timestamps_id = -1;
   int max_initial_timestamp_index = 50;
   bool return_no_speech_prob = false;
+  // the sampler (decoding.cc:1067-1074): RandomSampler when sampling_topk != 1 and sampling_temperature != 0 (then beam_size 1
+  // and num_hypotheses independent samples per entry), BestSampler otherwise
+  int sampling_topk = 1;                  // 0 = the whole vocabulary
+  float sampling_temperature = 1.f;
 };
 // models::Whisper::align (include/ctranslate2/models/whisper.h:135-140, src/models/whisper.cc:424-582) on ids: every entry is
 // start + <|notimestamps|> + text + <|endoftext|>; heads = the (decoder layer, head) pairs of config.json's alignment_heads

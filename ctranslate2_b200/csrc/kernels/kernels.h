@@ -221,6 +221,15 @@ struct BeamState {
   int32_t* hyp_tokens = nullptr;    // [batch, max_hyp, stride]
   int32_t* hyp_len = nullptr;       // [batch, max_hyp]
   float* hyp_score = nullptr;       // [batch, max_hyp] cumulative log-probability (not normalised)
+  // Sampled search (GreedySearch with a RandomSampler, decoding.cc:751-971): sample_topk >= 0 selects it.  The `beam` rows of an
+  // entry are its num_hypotheses independent samples; ancestry stays the identity and hypothesis slot h belongs to row h.
+  int sample_topk = -1;             // 0 = the whole vocabulary
+  float sample_temperature = 1.f;
+  const uint32_t* rng = nullptr;    // [2] process seed, index of this sampling call (philox.h)
+  int32_t* sample_ids = nullptr;    // [N] the step's sampled ids
+  float* sample_logp = nullptr;     // [N] their log-probabilities
+  float* row_score = nullptr;       // [N] cumulative log-probability of the row
+  int32_t* row_done = nullptr;      // [N] the row's hypothesis is registered
 };
 void launch_beam_init(void* cum, int32_t* ids, int64_t rows, int beam, int start_id, int dtype, cudaStream_t st);
 void launch_beam_logprobs(void* logits, const void* cum, const BeamState& s, int dtype, cudaStream_t st);
@@ -230,6 +239,14 @@ void launch_beam_rows(void* logits, const void* cum, const BeamState& s, void* r
                       cudaStream_t st);
 // one prompt position without a search step: next ids = forced_next [rows], identity ancestry, step + 1
 void launch_beam_force(const BeamState& s, const int32_t* forced_next, cudaStream_t st);
+// sampled search step (s.sample_topk >= 0): beam_mask_row + RandomSampler::sample on every row of logits (modified in place)
+// -> s.sample_ids / s.sample_logp, then the update: histories, row scores, hypothesis h of a row that ends, step + 1
+void launch_beam_sample(void* logits, const BeamState& s, int dtype, cudaStream_t st);
+void launch_beam_sample_update(const BeamState& s, cudaStream_t st);
+// RandomSampler::sample on rows x [rows, ld] T of `vocab` logits: ids [rows], logp [rows] = T(LogSoftMax(x))[id]; the
+// uniform of row r is philox_uniform(seed, call, r, step) (philox.h)
+void launch_random_sample(const void* x, int64_t rows, int64_t vocab, int64_t ld, int k, float temperature, uint32_t seed,
+                          uint32_t call, uint32_t step, int32_t* ids, float* logp, int dtype, cudaStream_t st);
 // out[r] = softmax(logits[r * row_stride : +vocab])[token]
 void launch_token_prob(const void* logits, int64_t rows, int64_t vocab, int64_t row_stride, int token, float* out, int dtype,
                        cudaStream_t st);

@@ -11,6 +11,8 @@
 #include "../common.cuh"
 #include "beam_decide.h"
 #include "kernels.h"
+#include "philox.h"
+#include "sample_row.cuh"
 
 namespace ct2b200 {
 
@@ -746,6 +748,82 @@ __global__ void beam_force_kernel(BeamState st, const int32_t* __restrict__ forc
   }
 }
 
+// GreedySearch::search with a RandomSampler (decoding.cc:844-971), one CTA per row: the row's DisableTokens / timestamp rules,
+// then the draw.  The seed and the call index come from device memory, so a replayed graph draws fresh numbers.
+template <typename T>
+__global__ void __launch_bounds__(kSampleThreads) beam_sample_kernel(T* __restrict__ logits, BeamState st) {
+  __shared__ SampleShared sm;
+  __shared__ int s_check;
+  griddep_launch();
+  griddep_wait();
+  const int64_t row = blockIdx.x;
+  const int step = *st.step;
+  T* xr = logits + row * st.vocab_ld;
+  beam_mask_row(xr, st, row, step, sm.red, &s_check);
+  const float u = philox_uniform(st.rng[0], st.rng[1], static_cast<uint32_t>(row), static_cast<uint32_t>(step));
+  sample_row(xr, st.vocab, st.sample_topk, st.sample_temperature, u, sm, st.sample_ids + row, st.sample_logp + row);
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kSampleThreads) random_sample_kernel(const T* __restrict__ x, int vocab, int64_t ld, int k,
+                                                                       float temperature, uint32_t seed, uint32_t call,
+                                                                       uint32_t step, int32_t* __restrict__ ids,
+                                                                       float* __restrict__ logp) {
+  __shared__ SampleShared sm;
+  const int64_t row = blockIdx.x;
+  const float u = philox_uniform(seed, call, static_cast<uint32_t>(row), step);
+  sample_row(x + row * ld, vocab, k, temperature, u, sm, ids + row, logp + row);
+}
+
+// The bookkeeping of the sampled search, one thread per row (results[batch_id] of decoding.cc:910-960, with every entry
+// repeated num_hypotheses times): the token joins the row's history, its log-probability the row's score; a row that samples
+// an end token or reaches the last step registers hypothesis h (the end token counted in the score, left out of the
+// hypothesis per include_eos).  An entry is finished when its rows all are.  The last CTA advances the step.
+__global__ void beam_sample_update_kernel(BeamState st) {
+  const int N = st.batch * st.beam, L = st.stride;
+  const int n = blockIdx.x * blockDim.x + threadIdx.x;
+  const int step = *st.step, rel = step - st.start_step;
+  if (n < N) {
+    const int i = n / st.beam, h = n % st.beam;
+    const int32_t tok = st.sample_ids[n];
+    int32_t* hist0 = st.alive + static_cast<int64_t>(n) * L;
+    int32_t* hist1 = hist0 + static_cast<int64_t>(N) * L;
+    hist0[rel] = tok;                                  // identity ancestry: both parities hold the whole history
+    hist1[rel] = tok;
+    st.anc[static_cast<int64_t>(n) * L + step] = n;
+    st.anc[static_cast<int64_t>(N) * L + static_cast<int64_t>(n) * L + step] = n;
+    st.next_ids[n] = tok;
+    if (!st.row_done[n]) {
+      const float score = st.row_score[n] + st.sample_logp[n];
+      st.row_score[n] = score;
+      bool is_end = false;
+      for (int e = 0; e < st.num_end; ++e) is_end |= st.end_ids[e] == tok;
+      if (is_end || rel + 1 >= st.max_steps) {
+        const int len = (is_end && !st.include_eos) ? rel : rel + 1;
+        int32_t* dst = st.hyp_tokens + (static_cast<int64_t>(i) * st.max_hyp + h) * L;
+        for (int t = 0; t < len; ++t) dst[t] = hist0[t];
+        st.hyp_len[i * st.max_hyp + h] = len;
+        st.hyp_score[i * st.max_hyp + h] = score;
+        st.row_done[n] = 1;
+        __threadfence();
+        if (atomicAdd(st.num_hyp + i, 1) == st.beam - 1) {
+          st.finished[i] = 1;
+          atomicAdd(st.num_finished, 1);
+        }
+      }
+    }
+  }
+  __threadfence();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const bool last = atomicAdd(st.ticket, 1) == static_cast<int>(gridDim.x) - 1;
+    if (last) {
+      *st.ticket = 0;
+      *st.step = step + 1;
+    }
+  }
+}
+
 // probability of one token under ops::SoftMax of the row (get_no_speech_probs_from_logits, models/whisper.cc:131-147)
 template <typename T>
 __global__ void __launch_bounds__(256) token_prob_kernel(const T* __restrict__ logits, int64_t vocab, int64_t row_stride,
@@ -1064,6 +1142,30 @@ void launch_beam_rows(void* logits, const void* cum, const BeamState& s, void* r
 void launch_beam_force(const BeamState& s, const int32_t* forced_next, cudaStream_t st) {
   const int rows = s.batch * s.beam;
   beam_force_kernel<<<div_up(rows, 128), 128, 0, st>>>(s, forced_next);
+  check_launch();
+}
+
+void launch_beam_sample(void* logits, const BeamState& s, int dtype, cudaStream_t st) {
+  const int64_t rows = static_cast<int64_t>(s.batch) * s.beam;
+  CT2_REQUIRE(s.sample_topk >= 0 && s.sample_topk <= s.vocab && s.sample_temperature > 0.f, "beam_sample: bad sampler");
+  CT2_DISPATCH_DTYPE(dtype, (launch_pdl(beam_sample_kernel<T>, dim3(rows), dim3(kSampleThreads), 0, st, static_cast<T*>(logits),
+                                        s)));
+}
+
+void launch_beam_sample_update(const BeamState& s, cudaStream_t st) {
+  const int rows = s.batch * s.beam;
+  beam_sample_update_kernel<<<div_up(rows, 128), 128, 0, st>>>(s);
+  check_launch();
+}
+
+void launch_random_sample(const void* x, int64_t rows, int64_t vocab, int64_t ld, int k, float temperature, uint32_t seed,
+                          uint32_t call, uint32_t step, int32_t* ids, float* logp, int dtype, cudaStream_t st) {
+  CT2_REQUIRE(vocab >= 1 && vocab <= INT32_MAX && ld >= vocab, "random_sample: bad row shape");
+  CT2_REQUIRE(k >= 0 && k <= vocab, "random_sample: sampling_topk must be in [0, vocab]");
+  CT2_REQUIRE(temperature > 0.f, "random_sample: the temperature must be positive");
+  if (rows == 0) return;
+  CT2_DISPATCH_DTYPE(dtype, (random_sample_kernel<T><<<static_cast<unsigned>(rows), kSampleThreads, 0, st>>>(
+                                static_cast<const T*>(x), static_cast<int>(vocab), ld, k, temperature, seed, call, step, ids, logp)));
   check_launch();
 }
 

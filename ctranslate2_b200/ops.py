@@ -256,6 +256,30 @@ class TopK:
         return v, i
 
 
+def random_sample(logits, k: int, temperature: float, seed: int, counter: int, step: int = 0):
+    """RandomSampler::sample on every row of logits [..., vocab]: keep the top k (0 = all), divide by the temperature, draw
+    one id by inverse CDF against u = philox_uniform(seed, counter, row, step) (csrc/kernels/philox.h).  Returns (ids int32,
+    log-probabilities f32 of the unscaled rows at those ids)."""
+    x = _c(logits)
+    cols = x.shape[-1]
+    rows = x.numel() // cols
+    ids = torch.empty(x.shape[:-1], dtype=torch.int32, device=x.device)
+    logp = torch.empty(x.shape[:-1], dtype=torch.float32, device=x.device)
+    check(lib().ct2b200_random_sample(_p(x), ctypes.c_int64(rows), ctypes.c_int64(cols), int(k), ctypes.c_float(temperature),
+                                      ctypes.c_uint32(seed), ctypes.c_uint32(counter), ctypes.c_uint32(step), _p(ids),
+                                      _p(logp), _dt(x), _stream()))
+    return ids, logp
+
+
+def philox4x32_10(counter, key):
+    """Philox4x32-10 of four 32-bit counter words under two key words, computed on the host by the library's own code."""
+    c = (ctypes.c_uint32 * 4)(*[int(v) & 0xFFFFFFFF for v in counter])
+    k = (ctypes.c_uint32 * 2)(*[int(v) & 0xFFFFFFFF for v in key])
+    out = (ctypes.c_uint32 * 4)()
+    check(lib().ct2b200_philox4x32_host(c, k, out))
+    return list(out)
+
+
 class Gather:
     """ops::Gather(axis=0, batch_dims=0)(data, ids) -> rows."""
     def __init__(self, axis: int = 0, batch_dims: int = 0):

@@ -110,10 +110,22 @@ class Whisper:
                  max_initial_timestamp_index: int = 50, suppress_blank: bool = True,
                  suppress_tokens: Sequence[int] = (-1,), sampling_topk: int = 1,
                  sampling_temperature: float = 1.0) -> List[WhisperGenerationResult]:
-        if repetition_penalty != 1 or no_repeat_ngram_size != 0 or return_logits_vocab or sampling_topk != 1 \
-                or sampling_temperature != 1:
-            raise ValueError("this engine implements the default repetition_penalty, no_repeat_ngram_size, return_logits_vocab, "
-                             "sampling_topk and sampling_temperature only")
+        """Whisper::generate.  sampling_topk != 1 with sampling_temperature != 0 selects random sampling (decoding.cc:1067-1074):
+        beam_size must be 1, and each entry returns num_hypotheses (<= 32) independent samples, best first; the draws follow
+        set_random_seed.  Otherwise the search is deterministic and the sampling options have no effect."""
+        if repetition_penalty != 1 or no_repeat_ngram_size != 0 or return_logits_vocab:
+            raise ValueError("this engine implements the default repetition_penalty, no_repeat_ngram_size and "
+                             "return_logits_vocab only")
+        sampling_topk, sampling_temperature = int(sampling_topk), float(sampling_temperature)
+        if sampling_topk < 0 or sampling_temperature < 0:
+            raise ValueError("sampling_topk and sampling_temperature must be >= 0")
+        sampling = sampling_topk != 1 and sampling_temperature != 0
+        if sampling and sampling_topk > self.vocab_size:         # checked by RandomSampler::sample only (sampling.cc:53-58)
+            raise ValueError("sampling_topk option (%d) is greater than the vocabulary size (%d)" % (sampling_topk, self.vocab_size))
+        if sampling and beam_size != 1:
+            raise ValueError("random sampling with beam_size > 1 (sampled beam search) is not supported: use beam_size=1")
+        if sampling and not 1 <= num_hypotheses <= 32:
+            raise ValueError("num_hypotheses must be in [1, 32] when sampling")
         f = self._features(features)
         rows = [[self._ids[t] if isinstance(t, str) else int(t) for t in r] for r in prompts]
         if not rows:
@@ -138,13 +150,17 @@ class Whisper:
         scores = np.zeros((B, num_hypotheses), np.float32)
         nsp = np.zeros(B, np.float32)
         p = ctypes.c_void_p
-        check(lib().ct2b200_whisper_generate(
-            p(self._h), f.ctypes.data_as(p), ctypes.c_int64(B), ctypes.c_int64(T), pr.ctypes.data_as(p), ctypes.c_int64(P),
-            int(beam_size), ctypes.c_float(patience), ctypes.c_float(length_penalty), ctypes.c_int64(max_length),
-            int(num_hypotheses), sup.ctypes.data_as(p), int(sup.size), beg.ctypes.data_as(p), int(beg.size),
-            ctypes.c_int32(self.sot_id), ctypes.c_int32(self.eot_id), ctypes.c_int32(self.no_speech_id),
-            ctypes.c_int32(self.no_timestamps_id), int(max_initial_timestamp_index), out.ctypes.data_as(p),
-            lens.ctypes.data_as(p), scores.ctypes.data_as(p), nsp.ctypes.data_as(p) if return_no_speech_prob else None))
+        args = [p(self._h), f.ctypes.data_as(p), ctypes.c_int64(B), ctypes.c_int64(T), pr.ctypes.data_as(p), ctypes.c_int64(P),
+                int(beam_size), ctypes.c_float(patience), ctypes.c_float(length_penalty), ctypes.c_int64(max_length),
+                int(num_hypotheses), sup.ctypes.data_as(p), int(sup.size), beg.ctypes.data_as(p), int(beg.size),
+                ctypes.c_int32(self.sot_id), ctypes.c_int32(self.eot_id), ctypes.c_int32(self.no_speech_id),
+                ctypes.c_int32(self.no_timestamps_id), int(max_initial_timestamp_index)]
+        outs = [out.ctypes.data_as(p), lens.ctypes.data_as(p), scores.ctypes.data_as(p),
+                nsp.ctypes.data_as(p) if return_no_speech_prob else None]
+        if sampling:
+            check(lib().ct2b200_whisper_generate_sampling(*args, sampling_topk, ctypes.c_float(sampling_temperature), *outs))
+        else:
+            check(lib().ct2b200_whisper_generate(*args, *outs))
         results = []
         for b in range(B):
             ids = [out[b, h, :lens[b, h]].tolist() for h in range(num_hypotheses) if lens[b, h] >= 0]

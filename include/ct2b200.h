@@ -154,6 +154,19 @@ CT2B200_API int ct2b200_log_softmax_gather(const void* x_d, const int32_t* ids_d
 CT2B200_API int ct2b200_topk(const void* x_d, int64_t rows, int64_t cols, int k, void* values_d, int32_t* indices_d,
                  int dtype, void* stream);
 
+/* RandomSampler::sample (src/sampling.cc:34-101) on rows x_d [rows, cols] T: keep the top k of the row (value desc, index asc;
+ * k = 0 or k = cols keeps all), weights exp((x - max) / temperature), one draw by inverse CDF in ascending index order against
+ * u * sum, where u = philox_uniform(seed, counter, row, step) (csrc/kernels/philox.h).  ids_d int32 [rows] = the drawn ids,
+ * logp_d f32 [rows] = T(LogSoftMax(x))[id], the log-probability of the unscaled row.  k in [0, cols], temperature > 0. */
+CT2B200_API int ct2b200_random_sample(const void* x_d, int64_t rows, int64_t cols, int k, float temperature, uint32_t seed,
+                                      uint32_t counter, uint32_t step, int32_t* ids_d, float* logp_d, int dtype, void* stream);
+/* set_random_seed (src/random.cc): the process-wide seed of sampled searches; also resets the sampling-call counter, so the
+ * same sequence of calls after the same seed gives the same results.  Without it a seed is drawn once from
+ * std::random_device. */
+CT2B200_API int ct2b200_set_random_seed(uint32_t seed);
+/* Host only (no device): Philox4x32-10 of counter_h [4] under key_h [2] -> out_h [4], the generator of the sampling kernels. */
+CT2B200_API int ct2b200_philox4x32_host(const uint32_t* counter_h, const uint32_t* key_h, uint32_t* out_h);
+
 /* ops::Gather::compute<Device::CUDA,T>(axis 0) — src/ops/gather_gpu.cu:52-91.  Row copy of `row_bytes`. */
 CT2B200_API int ct2b200_gather_rows(const void* data_d, const int32_t* ids_d, int64_t num_ids, int64_t row_bytes,
                         void* out_d, void* stream);
@@ -447,6 +460,22 @@ CT2B200_API int ct2b200_whisper_generate(ct2b200_translator* t, const float* fea
                              const int32_t* suppress_begin_h, int num_begin, int32_t sot_id, int32_t eot_id,
                              int32_t no_speech_id, int32_t no_timestamps_id, int max_initial_timestamp_index,
                              int32_t* out_ids_h, int32_t* out_lens_h, float* out_scores_h, float* no_speech_h);
+/* Whisper::generate with WhisperOptions::sampling_topk / sampling_temperature (src/models/whisper.cc:296-310, the sampler
+ * choice of decoding.cc:1067-1074): the arguments of ct2b200_whisper_generate, plus the sampler.  sampling_topk == 1 or
+ * sampling_temperature == 0 is the search of ct2b200_whisper_generate.  Otherwise beam_size must be 1 and every entry decodes
+ * num_hypotheses (<= 32) independent sampled rows (GreedySearch, decoding.cc:751-971): each step keeps the top sampling_topk
+ * (0 = all) of the processed logits, divides by the temperature and draws one token (ct2b200_random_sample, seeded by
+ * ct2b200_set_random_seed); a row's score is the sum of the log-probabilities of its tokens (the end token included) over
+ * length^length_penalty, and the rows of an entry come back best first.  sampling_topk in [0, vocab],
+ * sampling_temperature >= 0. */
+CT2B200_API int ct2b200_whisper_generate_sampling(ct2b200_translator* t, const float* features_h, int64_t batch, int64_t frames,
+                                                  const int32_t* prompts_h, int64_t prompt_len, int beam_size, float patience,
+                                                  float length_penalty, int64_t max_length, int num_hypotheses,
+                                                  const int32_t* suppress_ids_h, int num_suppress, const int32_t* suppress_begin_h,
+                                                  int num_begin, int32_t sot_id, int32_t eot_id, int32_t no_speech_id,
+                                                  int32_t no_timestamps_id, int max_initial_timestamp_index, int sampling_topk,
+                                                  float sampling_temperature, int32_t* out_ids_h, int32_t* out_lens_h,
+                                                  float* out_scores_h, float* no_speech_h);
 /* Whisper::align(features, start_sequence, text_tokens, num_frames, median_filter_width) — include/ctranslate2/models/whisper.h:
  * 135-140, src/models/whisper.cc:387-582: word-level timings from the cross-attention of the alignment heads.  Every entry is
  * start + <|notimestamps|> + text + <|endoftext|>, run through the decoder in one teacher-forced pass (the memory unmasked).

@@ -487,8 +487,63 @@ def make_whisper_align_fixture():
     print("whisper align fixture:", sum(len(m["cases"]) for m in fixture["models"].values()), "cases")
 
 
+WHISPER_SAMPLING_SEED = 2024
+
+
+def whisper_sampling_cases():
+    """(features seed, prompt, sampling_topk, sampling_temperature, num_hypotheses, length_penalty) on tiny_whisper, batch 2,
+    max_length 24: k in {0, 5}, T in {0.5, 1.0, 1.5}, H in {1, 3}, length penalties 0 and 1, with and without timestamps."""
+    cases, seed = [], 430
+    for prompt in ([101, 102, 106, 110], [101, 102, 106]):
+        for k in (0, 5):
+            for t in (0.5, 1.0, 1.5):
+                for h in (1, 3):
+                    for lp in (0.0, 1.0):
+                        cases.append((seed, prompt, k, t, h, lp))
+                        seed += 1
+    return cases
+
+
+def make_whisper_sampling_fixture():
+    """models::Whisper::generate with a RandomSampler of the UNMODIFIED reference (oracle/_ref, CPU, float32) on tiny_whisper
+    through tools/ref_whisper_sample.cc: the sampled sequences and their scores (no RNG parity: the tests check the score
+    convention of these sequences and their top-k membership, not the draws).  Features are re-generated from their seeds."""
+    import subprocess
+    import tempfile
+    out_dir = os.path.join(tempfile.gettempdir(), "ct2ref_sample")
+    subprocess.run(["make", "-s", "-f", "tools/ref_whisper_sample.mk", "sample", "SAMPLE_OUT=" + out_dir], cwd=ROOT, check=True)
+    cases, lines = whisper_sampling_cases(), []
+    for i, (seed, prompt, k, t, h, lp) in enumerate(cases):
+        path = os.path.join(out_dir, "features_%d.f32" % i)
+        whisper_inputs(seed, 2, 16, 60).astype(np.float32).tofile(path)
+        lines.append("\t".join([path, "2 16 60", ";".join([" ".join(map(str, prompt))] * 2), str(k), repr(t), str(h), repr(lp),
+                                "24"]))
+    text = "%s\tfloat32\t%d\n" % (os.path.join(OUT, "tiny_whisper"), WHISPER_SAMPLING_SEED) + "".join(x + "\n" for x in lines)
+    out = subprocess.run([os.path.join(out_dir, "ref_whisper_sample")], input=text.encode(), capture_output=True,
+                         check=True).stdout.decode().split("\n")
+    fixture = {"n_mels": 16, "frames": 60, "batch": 2, "max_length": 24, "compute_type": "float32",
+               "seed": WHISPER_SAMPLING_SEED, "cases": []}
+    k_line = 0
+    for seed, prompt, k, t, h, lp in cases:
+        assert out[k_line] == "ok", out[k_line]
+        rows = out[k_line + 1:k_line + 1 + 2 * h]
+        k_line += 1 + 2 * h
+        hyps = [[] for _ in range(2)]
+        for r in rows:
+            b, score, ids = r.split("\t")
+            hyps[int(b)].append({"score": float(score), "ids": [int(x) for x in ids.split(" ")] if ids else []})
+        fixture["cases"].append({"seed": seed, "prompt": prompt, "sampling_topk": k, "sampling_temperature": t,
+                                 "num_hypotheses": h, "length_penalty": lp, "results": hyps})
+    with open(os.path.join(OUT, "whisper_sampling_ref.json"), "w") as f:
+        json.dump(fixture, f)
+    print("whisper sampling fixture:", len(fixture["cases"]), "cases")
+
+
 def main():
     os.makedirs(OUT, exist_ok=True)
+    if "--whisper-sampling-only" in sys.argv:
+        make_whisper_sampling_fixture()
+        return
     if "--whisper-align-only" in sys.argv:
         make_whisper_align_fixture()
         return
@@ -584,6 +639,7 @@ def main():
     make_translator_score_fixture()
     make_whisper_fixture()
     make_whisper_align_fixture()
+    make_whisper_sampling_fixture()
     print("done")
 
 
