@@ -33,6 +33,7 @@ namespace {
 using namespace tc;
 using namespace dec;
 
+// The accumulators are parked for the epilogue in the operand ring: it has been consumed by then.
 template <int BN, int NB>
 struct DecSmem {
   static constexpr int kA = NB * kTileM * kSwizzleBytes;       // weight bytes per stage (always 128-row slots)
@@ -40,7 +41,8 @@ struct DecSmem {
   static constexpr int kStage = kA + kB;
   static constexpr int kCtrl = 512;                            // barriers
   static constexpr int kAcc = acc_bytes(NB * BN);              // accumulators parked for the row-per-thread epilogue
-  static size_t bytes(int stages, int cs) { return kAcc + static_cast<size_t>(stages) * kStage + kCtrl + red_bytes(cs, NB, BN) + 1024; }
+  static __host__ __device__ int ring(int stages) { return stages * kStage > kAcc ? stages * kStage : kAcc; }
+  static size_t bytes(int stages, int cs) { return ring(stages) + kCtrl + red_bytes(cs, NB, BN) + 1024; }
 };
 
 // T = output dtype, KIND = 0 s8 / 1 f16 / 2 bf16, BN = wgmma N (activation rows, zero padded), NB = 2 for gate+up,
@@ -56,9 +58,9 @@ __global__ void __launch_bounds__(kTcThreads, 2)
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int nstages = p.stages;
-  uint32_t* accs = reinterpret_cast<uint32_t*>(smem);                    // [NB * BN columns][kAccPitch]
-  uint8_t* ring = smem + S::kAcc;
-  uint8_t* ctrl = ring + nstages * S::kStage;
+  uint8_t* ring = smem;
+  uint32_t* accs = reinterpret_cast<uint32_t*>(smem);                    // [NB * BN columns][kAccPitch], after the K loop
+  uint8_t* ctrl = ring + S::ring(nstages);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(ctrl);               // [kMaxStages]
   uint64_t* empty_bar = full_bar + kMaxStages;                           // [kMaxStages]
   uint32_t* red = reinterpret_cast<uint32_t*>(ctrl + S::kCtrl);          // split-K exchange buffer (CS > 1)
@@ -102,6 +104,7 @@ __global__ void __launch_bounds__(kTcThreads, 2)
       wgmma_wait();
       if (lane == 0) mbar_arrive(empty_bar + s);       // this warp's share of the stage has been read
     }
+    epi_bar_sync();                                    // every warp has read its last stage: the ring becomes `accs`
 #pragma unroll
     for (int w = 0; w < NB; ++w) acc_store<BN>(acc[w], accs + w * BN * kAccPitch);
     epi_bar_sync();
@@ -110,11 +113,17 @@ __global__ void __launch_bounds__(kTcThreads, 2)
 }
 
 // ---- host side ----
+// Ring depth.  Single-weight Dense layers (QKV, out, down) size the ring so that two CTAs fit on one SM, where three
+// stages fit in 110 KB: the CTA of the next launch (programmatic dependent launch) then streams its weights while this
+// one drains its ring and runs its epilogue, and split-K plans may place two CTAs per SM.  The fused gate/up GEMM keeps
+// one CTA per SM with a ring of up to 200 KB: two co-resident gate/up CTAs of three stages each made the Llama-3-8B
+// decode step slower, single-weight ones made it faster (README, "Measured").
 template <int BN, int NB>
 int stages_for(int cs, int nkb) {
   using S = DecSmem<BN, NB>;
-  constexpr size_t cap = 200 * 1024;
-  int st = static_cast<int>((cap - S::kAcc - S::kCtrl - red_bytes(cs, NB, BN) - 1024) / S::kStage);
+  const size_t fixed = S::kCtrl + red_bytes(cs, NB, BN) + 1024;
+  int st = static_cast<int>((110 * 1024 - fixed) / S::kStage);
+  if (NB == 2 || st < 3 || S::bytes(st, cs) > 110 * 1024) st = static_cast<int>((200 * 1024 - fixed) / S::kStage);
   st = std::max(2, std::min(st, kMaxStages));
   return std::max(2, std::min(st, std::max(nkb, 2)));
 }
