@@ -4,6 +4,7 @@ There is no CPU or PyTorch fallback: importing works anywhere, every compute cal
 H100."""
 from . import ops  # noqa: F401
 from ._lib import Ct2B200Error, kernel_launch_count, lib, set_random_seed  # noqa: F401
+from .encoder import Encoder, EncoderForwardOutput, encoder_summary  # noqa: F401
 from .generator import GenerationResult, Generator, ScoringResult, model_summary  # noqa: F401
 from .translator import TranslationResult, Translator, translator_summary  # noqa: F401
 from .whisper import Whisper, WhisperAlignmentResult, WhisperGenerationResult  # noqa: F401

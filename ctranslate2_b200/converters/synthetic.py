@@ -560,3 +560,85 @@ def write_whisper_model(model_dir: str, cfg: WhisperConfig, quantization: str = 
               "suppress_ids_begin": [3, eot], "lang_ids": list(range(eot + 2, eot + 2 + cfg.languages)),
               "alignment_heads": [[cfg.decoder_layers - 1, 0]]}
     w.close(config, vocab)
+
+
+# ---------------------------------------------------------------------------------------------
+# Encoder-only directories (TransformerEncoderModelSpec revision 1, spec name TransformerEncoderSpec,
+# python/ctranslate2/specs/transformer_spec.py:771-812), laid out as the BertLoader emits them
+# (python/ctranslate2/converters/transformers.py:3295-3330): token and token-type embeddings merged by ADD, unscaled,
+# stored positions, layernorm_embedding, post-norm GELU layers, pooler_dense + Tanh.
+# ---------------------------------------------------------------------------------------------
+@dataclass
+class EncoderConfig:
+    num_layers: int = 12
+    num_heads: int = 12
+    d_model: int = 768
+    ffn_dim: int = 3072
+    vocab_size: int = 30522
+    type_vocab_size: int = 2               # 0 = one embedding table (no token types)
+    max_positions: int = 512
+    pre_norm: bool = False                 # pre-norm adds the final encoder/layer_norm
+    activation: int = 3                    # common_spec.Activation: RELU = 0, GELUTanh = 1, GELU = 3
+    pooler: bool = True
+    layernorm_embedding: bool = True
+    layer_norm_epsilon: float = 1e-12
+
+
+BERT_BASE = EncoderConfig()
+
+
+def write_encoder_model(model_dir: str, cfg: EncoderConfig, quantization: str = "int8", seed: int = 1234,
+                        init_std: float = 0.05, emb_std: float = 0.5) -> None:
+    """Writes a random-init TransformerEncoderSpec directory (model.bin v6 + config.json + vocabulary.json)."""
+    rng = np.random.default_rng(seed)
+    is_int8 = quantization.startswith("int8")
+    ftype = {"int8": "float32", "int8_float32": "float32", "int8_float16": "float16",
+             "int8_bfloat16": "bfloat16"}.get(quantization, quantization)
+    d = cfg.d_model
+    w = ModelWriter(model_dir, spec="TransformerEncoderSpec", revision=1)
+
+    def linear(prefix, n, k, std=init_std, bias=True):
+        wt = (rng.standard_normal((n, k), dtype=np.float32) * np.float32(std))
+        if is_int8:
+            q, scale = quantize_int8(wt)
+            w.add(prefix + "/weight", q, "int8")
+            w.add(prefix + "/weight_scale", scale, "float32")
+        else:
+            w.add(prefix + "/weight", wt, ftype)
+        if bias:
+            w.add(prefix + "/bias", (0.02 * rng.standard_normal(n)).astype(np.float32), ftype)
+
+    def norm(prefix):
+        w.add(prefix + "/gamma", (1.0 + 0.1 * rng.standard_normal(d)).astype(np.float32), ftype)
+        w.add(prefix + "/beta", (0.05 * rng.standard_normal(d)).astype(np.float32), ftype)
+
+    w.add("encoder/num_heads", np.int16(cfg.num_heads))
+    w.add("encoder/pre_norm", np.int8(cfg.pre_norm))
+    w.add("encoder/activation", np.int8(cfg.activation))
+    w.add("encoder/embeddings_merge", np.int8(1))             # ADD
+    w.add("encoder/scale_embeddings", np.int8(0))
+    if cfg.type_vocab_size:
+        linear("encoder/embeddings_0", cfg.vocab_size, d, std=emb_std, bias=False)
+        linear("encoder/embeddings_1", cfg.type_vocab_size, d, std=emb_std, bias=False)
+    else:
+        linear("encoder/embeddings", cfg.vocab_size, d, std=emb_std, bias=False)
+    w.add("encoder/position_encodings/encodings", (0.1 * rng.standard_normal((cfg.max_positions, d))).astype(np.float32), ftype)
+    if cfg.layernorm_embedding:
+        norm("encoder/layernorm_embedding")
+    if cfg.pre_norm:
+        norm("encoder/layer_norm")
+    for l in range(cfg.num_layers):
+        p = f"encoder/layer_{l}"
+        norm(p + "/self_attention/layer_norm")
+        linear(p + "/self_attention/linear_0", 3 * d, d)
+        linear(p + "/self_attention/linear_1", d, d)
+        norm(p + "/ffn/layer_norm")
+        linear(p + "/ffn/linear_0", cfg.ffn_dim, d)
+        linear(p + "/ffn/linear_1", d, cfg.ffn_dim)
+    if cfg.pooler:
+        linear("pooler_dense", d, d)
+        w.add("pooler_activation", np.int8(5))                  # Tanh
+    config = {"unk_token": "[UNK]", "bos_token": "[CLS]", "eos_token": "[SEP]", "multi_query_attention": False,
+              "layer_norm_epsilon": cfg.layer_norm_epsilon}
+    vocab = ["[PAD]", "[UNK]", "[CLS]", "[SEP]"] + [f"<t{i}>" for i in range(4, cfg.vocab_size)]
+    w.close(config, vocab)

@@ -67,6 +67,9 @@ struct ct2b200_generator {
 struct ct2b200_translator {
   std::unique_ptr<Translator> impl;
 };
+struct ct2b200_encoder {
+  std::unique_ptr<Translator> impl;   // the encoder engine of the Translator in its encoder-only mode
+};
 
 extern "C" {
 
@@ -318,6 +321,16 @@ CT2B200_API int ct2b200_attention_encoder(const void* qkv, const int32_t* length
     require_device();
     CT2_REQUIRE(batch >= 0 && keys >= 0 && H > 0 && D > 0, "attention_encoder: bad shape");
     launch_attention_encoder(qkv, lengths, batch, keys, H, D, scale, out, dtype, S(stream));
+  });
+}
+
+CT2B200_API int ct2b200_attention_encoder_mma(const void* qkv, const int32_t* lengths, int64_t batch, int keys, int H, int D,
+                                              float scale, void* out, int dtype, void* stream) {
+  return guarded([&] {
+    require_device();
+    CT2_REQUIRE(batch >= 0 && keys >= 0 && H > 0 && D > 0, "attention_encoder_mma: bad shape");
+    if (!launch_attention_encoder_mma(qkv, lengths, batch, keys, H, D, scale, out, dtype, S(stream)))
+      throw std::invalid_argument("attention_encoder_mma: fp16 / bf16 with head_dim 64 or 128 only");
   });
 }
 
@@ -729,6 +742,62 @@ CT2B200_API int ct2b200_bench_translate(ct2b200_translator* t, int64_t batch, in
   return guarded([&] {
     CT2_REQUIRE(t && encode_ms && decode_ms && kernel_launches, "bench_translate: null argument");
     t->impl->bench(batch, source_len, beam_size, steps, warmup, encode_ms, decode_ms, kernel_launches);
+  });
+}
+
+// ---- Encoder ----
+CT2B200_API ct2b200_encoder* ct2b200_encoder_open(const char* model_dir, const ct2b200_generator_config* config) {
+  ct2b200_encoder* e = nullptr;
+  const int rc = guarded([&] {
+    require_device();
+    CT2_REQUIRE(model_dir && config, "encoder_open: null argument");
+    auto holder = std::make_unique<ct2b200_encoder>();
+    holder->impl = std::make_unique<Translator>(model_dir, *config, true);
+    e = holder.release();
+  });
+  return rc == 0 ? e : nullptr;
+}
+
+CT2B200_API void ct2b200_encoder_close(ct2b200_encoder* e) { delete e; }
+
+CT2B200_API int ct2b200_encoder_summary(const char* model_dir, char* json_out, size_t capacity) {
+  return guarded([&] {
+    CT2_REQUIRE(model_dir && json_out && capacity > 0, "encoder_summary: null argument");
+    ModelFile file(model_dir);
+    const Seq2SeqConfig mc = parse_encoder_config(file);
+    const HostVariable& pos = file.get("encoder/position_encodings/encodings");
+    char buf[1024];
+    const int n = std::snprintf(
+        buf, sizeof(buf),
+        "{\"spec\": \"%s\", \"binary_version\": %u, \"revision\": %u, \"num_layers\": %d, \"num_heads\": %d, "
+        "\"head_dim\": %d, \"d_model\": %lld, \"ffn_dim\": %lld, \"vocab_size\": %lld, \"type_vocab_size\": %lld, "
+        "\"max_positions\": %lld, \"weights\": \"%s\", \"pre_norm\": %s, \"activation\": %d, \"embeddings_scale\": %.9g, "
+        "\"layernorm_embedding\": %s, \"final_norm\": %s, \"pooler\": %s, \"pooler_activation\": %d, "
+        "\"layer_norm_epsilon\": %.9g, \"round_before_cast\": %s}",
+        file.spec_name.c_str(), file.binary_version, file.revision, mc.enc_layers, mc.num_heads, mc.head_dim,
+        static_cast<long long>(mc.d_model), static_cast<long long>(mc.ffn_dim), static_cast<long long>(mc.src_vocab),
+        static_cast<long long>(mc.type_vocab), static_cast<long long>(pos.shape[0]), mc.weights.c_str(),
+        mc.enc_pre_norm ? "true" : "false", mc.enc_activation, static_cast<double>(mc.enc_emb_scale),
+        mc.has_emb_norm ? "true" : "false", mc.has_enc_final_norm ? "true" : "false", mc.has_pooler ? "true" : "false",
+        mc.pooler_activation, static_cast<double>(mc.eps), mc.round_before_cast ? "true" : "false");
+    CT2_REQUIRE(n > 0 && static_cast<size_t>(n) < capacity, "encoder_summary: output buffer too small");
+    std::memcpy(json_out, buf, static_cast<size_t>(n) + 1);
+  });
+}
+
+CT2B200_API int ct2b200_encoder_forward(ct2b200_encoder* e, const int32_t* ids, const int32_t* lengths, const int32_t* token_type_ids,
+                                        int64_t batch, int64_t max_length, float* last_hidden_state, float* pooler_output) {
+  return guarded([&] {
+    CT2_REQUIRE(e && ids && lengths && last_hidden_state, "encoder_forward: null argument");
+    e->impl->encoder_forward(ids, token_type_ids, lengths, batch, max_length, last_hidden_state, pooler_output);
+  });
+}
+
+CT2B200_API int ct2b200_encoder_bench(ct2b200_encoder* e, const int32_t* lengths, int64_t batch, int64_t max_length, int64_t iters,
+                                      int64_t warmup, float* median_ms) {
+  return guarded([&] {
+    CT2_REQUIRE(e && lengths && median_ms, "encoder_bench: null argument");
+    e->impl->encoder_bench(lengths, batch, max_length, iters, warmup, median_ms);
   });
 }
 

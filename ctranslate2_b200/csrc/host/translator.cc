@@ -131,6 +131,71 @@ Seq2SeqConfig parse_seq2seq_config(const ModelFile& f) {
   return mc;
 }
 
+// TransformerEncoderModelSpec (python/ctranslate2/specs/transformer_spec.py:771-812) read as TransformerEncoder
+// (transformer.cc:405-471) + EncoderReplica's pooler (language_model.cc:335-345)
+Seq2SeqConfig parse_encoder_config(const ModelFile& f) {
+  Seq2SeqConfig mc;
+  mc.encoder_only = true;
+  if (f.spec_name != "TransformerEncoderSpec" || !f.find("encoder/layer_0/self_attention/linear_0/weight"))
+    throw std::invalid_argument("ct2b200 Encoder serves Transformer encoder models (TransformerEncoderSpec); got " + f.spec_name);
+  while (f.find("encoder/layer_" + std::to_string(mc.enc_layers) + "/self_attention/linear_0/weight")) ++mc.enc_layers;
+  auto absent = [&](const std::string& name, const char* what) {
+    if (f.find(name)) throw std::invalid_argument(std::string(what) + " (" + name + ") is not supported by the Encoder engine");
+  };
+  // ParallelEmbeddings (common.cc:84-148): one table, or the tokens and their types merged by ADD
+  const bool parallel = f.find("encoder/embeddings_0/weight") != nullptr;
+  const HostVariable& emb = f.get(parallel ? "encoder/embeddings_0/weight" : "encoder/embeddings/weight");
+  mc.src_vocab = emb.shape[0];
+  mc.d_model = emb.shape[1];
+  if (parallel) {
+    absent("encoder/embeddings_2/weight", "more than two input features");
+    if (const HostVariable* types = f.find("encoder/embeddings_1/weight")) {
+      if (f.attribute("encoder/embeddings_merge", 0.0) != 1.0)
+        throw std::invalid_argument("embeddings_merge CONCAT is not supported by the Encoder engine (ADD is)");
+      CT2_REQUIRE(types->shape.size() == 2 && types->shape[1] == mc.d_model, "token-type embeddings must have the model depth");
+      mc.type_vocab = types->shape[0];
+    }
+  }
+  mc.num_heads = static_cast<int>(f.attribute("encoder/num_heads", 8.0));
+  CT2_REQUIRE(mc.num_heads > 0 && mc.d_model % mc.num_heads == 0, "d_model must be divisible by num_heads");
+  mc.head_dim = static_cast<int>(mc.d_model / mc.num_heads);
+  mc.enc_pre_norm = f.attribute("encoder/pre_norm", 1.0) != 0.0;
+  mc.enc_activation = static_cast<int>(f.attribute("encoder/activation", 0.0));
+  if (mc.enc_activation != CT2B200_ACT_RELU && mc.enc_activation != CT2B200_ACT_GELU && mc.enc_activation != CT2B200_ACT_GELU_TANH)
+    throw std::invalid_argument("the Encoder engine runs ReLU, GELU and GELUTanh feed-forward layers; got activation " +
+                                std::to_string(mc.enc_activation));
+  mc.enc_emb_scale = embeddings_scale(f, "encoder", mc.d_model);
+  mc.ffn_dim = f.get("encoder/layer_0/ffn/linear_0/weight").shape[0];
+  mc.round_before_cast = f.binary_version >= 5;
+  mc.has_enc_final_norm = f.find("encoder/layer_norm/gamma") != nullptr;
+  mc.has_emb_norm = f.find("encoder/layernorm_embedding/gamma") != nullptr;
+  mc.has_pooler = f.find("pooler_dense/weight") != nullptr;
+  mc.pooler_activation = static_cast<int>(f.attribute("pooler_activation", static_cast<double>(CT2B200_ACT_TANH)));
+  CT2_REQUIRE(mc.pooler_activation >= CT2B200_ACT_RELU && mc.pooler_activation <= CT2B200_ACT_SIGMOID, "unknown pooler_activation");
+  const bool has_beta = f.find("encoder/layer_0/self_attention/layer_norm/beta") != nullptr;
+  mc.eps = static_cast<float>(f.config_number("layer_norm_epsilon", has_beta ? 1e-5 : 1e-6));
+  CT2_REQUIRE(has_beta, "RMSNorm encoder models are not supported (LayerNorm with beta is)");
+  CT2_REQUIRE(f.find("encoder/position_encodings/encodings") != nullptr,
+              "the Encoder engine needs stored position encodings (encoder/position_encodings/encodings)");
+  const std::string a = "encoder/layer_0/self_attention/";
+  absent(a + "relative_position_keys", "relative position representations");
+  absent(a + "relative_asymmetric_position_keys", "relative position representations");
+  absent(a + "relative_attention_bias", "relative attention bias");
+  absent(a + "rotary_dim", "rotary embeddings");
+  absent(a + "num_heads_kv", "grouped-query or multi-query attention");   // multi_query_attention stores num_heads_kv = 1
+  absent(a + "head_dim", "a head_dim other than d_model / num_heads");
+  absent(a + "sliding_window", "sliding-window attention");
+  absent(a + "q_norm/gamma", "query / key normalisation");
+  absent(a + "queries_scale", "a custom queries_scale");
+  absent("encoder/sliding_window", "sliding-window attention");
+  absent("encoder/layer_0/ffn/linear_0_noact/weight", "gated feed-forward layers");
+  absent("encoder/layer_0/input_layer_norm/gamma", "pre-and-post layer norms");
+  const HostVariable& w = f.get("encoder/layer_0/self_attention/linear_0/weight");
+  mc.weights = w.type_id == 1 ? "int8" : w.type_id == 2 ? "int16" : w.type_id == 4 ? "float16" : w.type_id == 5 ? "bfloat16" : "float32";
+  CT2_REQUIRE(w.type_id != 2, "int16 models are not supported (convert with int8 or a float type)");
+  return mc;
+}
+
 // =============================================================================================
 // loading
 // =============================================================================================
@@ -169,7 +234,7 @@ std::vector<float> sinusoidal_positions(int64_t max_time, int64_t depth) {
 }
 }  // namespace
 
-Translator::Translator(const std::string& model_dir, const ct2b200_generator_config& cfg) {
+Translator::Translator(const std::string& model_dir, const ct2b200_generator_config& cfg, bool encoder_only) {
   device_ = cfg.device;
   CT2_CUDA_CHECK(cudaSetDevice(device_));
   int major = 0;
@@ -184,8 +249,13 @@ Translator::Translator(const std::string& model_dir, const ct2b200_generator_con
   CT2_REQUIRE(cfg.tp_size <= 1, "the Translator engine does not run tensor parallel");
 
   ModelFile f(model_dir);
-  mc_ = parse_seq2seq_config(f);
-  if (mc_.whisper) {
+  mc_ = encoder_only ? parse_encoder_config(f) : parse_seq2seq_config(f);
+  if (mc_.encoder_only) {
+    load_dense(f, f.find("encoder/embeddings_0/weight") ? "encoder/embeddings_0" : "encoder/embeddings", enc_emb_);
+    if (mc_.type_vocab) load_dense(f, "encoder/embeddings_1", type_emb_);
+    if (mc_.has_emb_norm) load_norm(f, "encoder/layernorm_embedding", emb_norm_);
+    if (mc_.has_pooler) load_dense(f, "pooler_dense", pooler_);
+  } else if (mc_.whisper) {
     // the convolutions run as im2col + float Dense: weights [d, Cin, 3] flattened to [d, Cin * 3] in T (the reference keeps
     // them in float on CUDA too, model.cc:204-223; an int8-stored convolution is dequantized here: w = q / scale)
     auto load_conv = [&](const std::string& prefix, DenseWeights& w) {
@@ -223,8 +293,10 @@ Translator::Translator(const std::string& model_dir, const ct2b200_generator_con
   } else {
     load_dense(f, embeddings_scope(f, "encoder"), enc_emb_);
   }
-  load_dense(f, "decoder/embeddings", dec_emb_);
-  load_dense(f, "decoder/projection", projection_);
+  if (!mc_.encoder_only) {
+    load_dense(f, "decoder/embeddings", dec_emb_);
+    load_dense(f, "decoder/projection", projection_);
+  }
   if (mc_.has_enc_final_norm) load_norm(f, "encoder/layer_norm", enc_norm_);
   if (mc_.has_dec_final_norm) load_norm(f, "decoder/layer_norm", dec_norm_);
   enc_.resize(mc_.enc_layers);
@@ -270,7 +342,7 @@ Translator::Translator(const std::string& model_dir, const ct2b200_generator_con
     return count;
   };
   enc_positions_ = load_positions("encoder", enc_pos_);
-  dec_positions_ = load_positions("decoder", dec_pos_);
+  if (!mc_.encoder_only) dec_positions_ = load_positions("decoder", dec_pos_);
   SplitKWorkspace::get(stream_);   // create the split-K scratch outside any graph capture
   CT2_CUDA_CHECK(cudaDeviceSynchronize());
 }
@@ -421,8 +493,12 @@ void Translator::run_encoder_layers(int64_t batch, int64_t S, const int32_t* len
   for (int l = 0; l < mc_.enc_layers; ++l) {
     EncoderLayerWeights& w = enc_[l];
     dense(w.self.in, pre ? &w.self.norm : nullptr, x_.ptr, rows, nullptr, -1, qkv_.ptr, xq);
-    launch_attention_encoder(qkv_.ptr, lens_d, batch, static_cast<int>(S), mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, dtype_,
-                             stream_);
+    // encoder-only models run the tensor-core kernel where it covers the shape; the Translator and Whisper encoders keep
+    // the generic one
+    if (!mc_.encoder_only || !launch_attention_encoder_mma(qkv_.ptr, lens_d, batch, static_cast<int>(S), mc_.num_heads,
+                                                           mc_.head_dim, scale, ctx_.ptr, dtype_, stream_))
+      launch_attention_encoder(qkv_.ptr, lens_d, batch, static_cast<int>(S), mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, dtype_,
+                               stream_);
     dense(w.self.out, nullptr, ctx_.ptr, rows, x_.ptr, -1, x_.ptr);
     xq = !pre && post_norm(w.self.norm, x_.ptr, rows, &w.ffn.ff1);
     dense(w.ffn.ff1, pre ? &w.ffn.norm : nullptr, x_.ptr, rows, nullptr, mc_.enc_activation, h_.ptr, xq);
@@ -775,6 +851,100 @@ void Translator::bench(int64_t batch, int64_t source_len, int beam, int64_t step
   cudaEventDestroy(e1);
   cudaEventDestroy(e2);
   cudaEventDestroy(e3);
+}
+
+// =============================================================================================
+// Encoder (models::EncoderReplica, src/models/language_model.cc:302-400)
+// =============================================================================================
+// TransformerEncoder::operator() with the merged embeddings (transformer.cc:427-471): tokens + types (ADD in T), scale,
+// positions, layernorm_embedding, the layers, output norm; then pooler_dense + activation on each row's first position
+void Translator::run_encoder_only(int64_t batch, int64_t S) {
+  const int64_t rows = batch * S, d = mc_.d_model;
+  launch_embed_pos(enc_emb_.weight.ptr, enc_emb_.kind == DenseWeights::INT8 ? enc_emb_.scale.as<float>() : nullptr,
+                   src_ids_.as<int32_t>(), rows, d, mc_.enc_emb_scale, enc_pos_.ptr, S, nullptr, false, x_.ptr, dtype_, stream_,
+                   mc_.type_vocab ? type_emb_.weight.ptr : nullptr,
+                   type_emb_.kind == DenseWeights::INT8 ? type_emb_.scale.as<float>() : nullptr, type_ids_.as<int32_t>());
+  if (mc_.has_emb_norm)
+    launch_layer_norm(x_.ptr, emb_norm_.gamma.ptr, emb_norm_.beta.ptr, rows, d, mc_.eps, x_.ptr, nullptr, nullptr, true, dtype_,
+                      stream_);
+  run_encoder_layers(batch, S, src_lens_.as<int32_t>());
+  if (mc_.has_pooler) {
+    const size_t es = dtype_size(dtype_);
+    CT2_CUDA_CHECK(cudaMemcpy2DAsync(first_.ptr, d * es, memory_.ptr, S * d * es, d * es, batch, cudaMemcpyDeviceToDevice, stream_));
+    dense(pooler_, nullptr, first_.ptr, batch, nullptr, mc_.pooler_activation, pooled_.ptr);
+  }
+}
+
+void Translator::encoder_forward(const int32_t* ids_h, const int32_t* types_h, const int32_t* lens_h, int64_t batch, int64_t T,
+                                 float* hidden_h, float* pooled_h) {
+  std::lock_guard<std::mutex> lock(mu_);
+  CT2_REQUIRE(mc_.encoder_only, "forward_batch needs an encoder model (TransformerEncoderSpec)");
+  CT2_REQUIRE(batch > 0 && T > 0, "forward_batch: empty batch");
+  CT2_REQUIRE(T <= enc_positions_, "forward_batch: the sequences are longer than the position table");
+  // padded positions get id 0 / type 0 so that every gathered row is in range
+  std::vector<int32_t> ids(batch * T, 0), types(batch * T, 0);
+  for (int64_t b = 0; b < batch; ++b) {
+    CT2_REQUIRE(lens_h[b] >= 1 && lens_h[b] <= T, "forward_batch: lengths must be in [1, max_length]");
+    for (int64_t t = 0; t < lens_h[b]; ++t) {
+      const int32_t id = ids_h[b * T + t];
+      CT2_REQUIRE(id >= 0 && id < mc_.src_vocab, "forward_batch: input id out of range");
+      ids[b * T + t] = id;
+      if (types_h) {
+        const int32_t ty = types_h[b * T + t];
+        CT2_REQUIRE(mc_.type_vocab > 0, "forward_batch: this model has no token-type embeddings");
+        CT2_REQUIRE(ty >= 0 && ty < mc_.type_vocab, "forward_batch: token type id out of range");
+        types[b * T + t] = ty;
+      }
+    }
+  }
+  ensure_rows(batch, batch * T, batch * T);
+  const size_t es = dtype_size(dtype_);
+  if (batch * T > cap_types_) {
+    cap_types_ = batch * T;
+    type_ids_.alloc(cap_types_ * 4);
+  }
+  if (mc_.has_pooler && batch > cap_pooled_) {
+    cap_pooled_ = batch;
+    first_.alloc(batch * mc_.d_model * es);
+    pooled_.alloc(batch * mc_.d_model * es);
+  }
+  CT2_CUDA_CHECK(cudaMemcpyAsync(src_ids_.ptr, ids.data(), ids.size() * 4, cudaMemcpyHostToDevice, stream_));
+  CT2_CUDA_CHECK(cudaMemcpyAsync(type_ids_.ptr, types.data(), types.size() * 4, cudaMemcpyHostToDevice, stream_));
+  CT2_CUDA_CHECK(cudaMemcpyAsync(src_lens_.ptr, lens_h, batch * 4, cudaMemcpyHostToDevice, stream_));
+  run_encoder_only(batch, T);
+  if (mc_.has_pooler && pooled_h) {
+    DeviceBuffer f32(static_cast<size_t>(batch) * mc_.d_model * 4);
+    launch_convert_to_f32(pooled_.ptr, batch * mc_.d_model, f32.as<float>(), dtype_, stream_);
+    CT2_CUDA_CHECK(cudaMemcpyAsync(pooled_h, f32.ptr, f32.bytes, cudaMemcpyDeviceToHost, stream_));
+    CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));
+  }
+  copy_memory_to_host(batch * T, hidden_h);     // synchronises: ids / types may go
+}
+
+void Translator::encoder_bench(const int32_t* lens_h, int64_t batch, int64_t T, int64_t iters, int64_t warmup, float* median_ms) {
+  CT2_REQUIRE(iters >= 1 && warmup >= 0, "encoder_bench: iters must be >= 1");
+  std::vector<int32_t> ids(batch * T), types(batch * T, 0);
+  for (size_t i = 0; i < ids.size(); ++i) ids[i] = static_cast<int32_t>((7919ull * i + 3) % mc_.src_vocab);
+  std::vector<float> hidden(static_cast<size_t>(batch) * T * mc_.d_model), pooled(static_cast<size_t>(batch) * mc_.d_model);
+  encoder_forward(ids.data(), mc_.type_vocab ? types.data() : nullptr, lens_h, batch, T, hidden.data(), pooled.data());
+  std::lock_guard<std::mutex> lock(mu_);
+  cudaEvent_t e0, e1;
+  cudaEventCreate(&e0);
+  cudaEventCreate(&e1);
+  std::vector<float> ms;
+  for (int64_t i = 0; i < warmup + iters; ++i) {
+    cudaEventRecord(e0, stream_);
+    run_encoder_only(batch, T);
+    cudaEventRecord(e1, stream_);
+    CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    float t = 0.f;
+    cudaEventElapsedTime(&t, e0, e1);
+    if (i >= warmup) ms.push_back(t);
+  }
+  cudaEventDestroy(e0);
+  cudaEventDestroy(e1);
+  std::sort(ms.begin(), ms.end());
+  *median_ms = ms[ms.size() / 2];
 }
 
 // =============================================================================================

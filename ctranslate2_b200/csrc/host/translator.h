@@ -27,11 +27,18 @@ struct Seq2SeqConfig {
   bool start_from_zero_embedding = false;            // Marian / OPUS-MT decoders (transformer.cc:637-640)
   bool whisper = false;                              // WhisperSpec: Conv1D front-end instead of source embeddings
   int64_t n_mels = 0, max_frames = 0;                // Whisper: input channels, encoder positions (frames / 2)
+  // TransformerEncoderSpec (models::EncoderReplica, language_model.cc:302-400): the encoder alone, no decoder
+  bool encoder_only = false;
+  int64_t type_vocab = 0;                            // rows of the token-type embeddings merged by ADD (0 = none)
+  bool has_emb_norm = false;                         // layernorm_embedding
+  bool has_pooler = false;                           // pooler_dense on the first position
+  int pooler_activation = CT2B200_ACT_TANH;
   int64_t weight_bytes = 0;
   std::string weights;                               // storage type of the linear layers
 };
 
 Seq2SeqConfig parse_seq2seq_config(const ModelFile& file);   // host only
+Seq2SeqConfig parse_encoder_config(const ModelFile& file);   // host only; TransformerEncoderSpec directories
 
 struct NormWeights {
   DeviceBuffer gamma, beta;
@@ -114,7 +121,8 @@ struct WhisperAlignResult {
 
 class Translator {
  public:
-  Translator(const std::string& model_dir, const ct2b200_generator_config& cfg);
+  // encoder_only: a TransformerEncoderSpec directory (parse_encoder_config), served by encoder_forward / encoder_bench only
+  Translator(const std::string& model_dir, const ct2b200_generator_config& cfg, bool encoder_only = false);
   ~Translator();
   const Seq2SeqConfig& config() const { return mc_; }
   int dtype() const { return dtype_; }
@@ -142,6 +150,14 @@ class Translator {
   // decoder position (input <|startoftranscript|>), in lang_ids order
   void whisper_detect_language(const float* features_h, int64_t batch, int64_t frames, int32_t sot_id,
                                const std::vector<int32_t>& lang_ids, float* probs_h);
+  // EncoderReplica::forward_impl (language_model.cc:349-400): ids_h / types_h (null: zeros) [batch, T] host, lens_h [batch]
+  // in [1, T]; hidden_h [batch, T, d_model] f32 (positions past a row's length unspecified), pooled_h [batch, d_model] f32
+  // (models with a pooler; ignored otherwise)
+  void encoder_forward(const int32_t* ids_h, const int32_t* types_h, const int32_t* lens_h, int64_t batch, int64_t T,
+                       float* hidden_h, float* pooled_h);
+  // device-timed encoder-only passes over resident inputs of `batch` rows of lens_h[b] <= T tokens: the median of `iters`
+  // passes after `warmup`
+  void encoder_bench(const int32_t* lens_h, int64_t batch, int64_t T, int64_t iters, int64_t warmup, float* median_ms);
   // device-timed phases for bench.py: encoder pass, then `steps` decoding steps of batch * beam rows
   void bench(int64_t batch, int64_t source_len, int beam, int64_t steps, int64_t warmup, float* encode_ms, float* decode_ms,
              int64_t* launches);
@@ -162,6 +178,8 @@ class Translator {
   bool post_norm(const NormWeights& n, void* x, int64_t rows, const DenseWeights* next);
   void run_encoder(int64_t batch, int64_t S);
   void run_encoder_layers(int64_t batch, int64_t S, const int32_t* lens_d);
+  // the encoder-only model on src_ids_ / type_ids_ / src_lens_ -> memory_, and the pooler on its first positions -> pooled_
+  void run_encoder_only(int64_t batch, int64_t S);
   // encoder positions of `frames` input frames; refuses a features shape the encoder cannot take
   int64_t whisper_positions(int64_t batch, int64_t frames) const;
   // the Whisper encoder on features_h [batch, n_mels, frames] f32 (host) -> memory_; src_lens_ = every position
@@ -202,6 +220,10 @@ class Translator {
   cudaStream_t stream_ = nullptr;
 
   DenseWeights enc_emb_, dec_emb_, projection_;
+  DenseWeights type_emb_, pooler_;   // encoder-only models: token-type embeddings, pooler_dense
+  NormWeights emb_norm_;             // encoder-only models: layernorm_embedding
+  DeviceBuffer type_ids_, first_, pooled_;   // token types [rows]; first positions / pooler output [entries, d_model]
+  int64_t cap_types_ = 0, cap_pooled_ = 0;
   DenseWeights conv1_, conv2_;   // Whisper: [d, n_mels * 3] / [d, d * 3] in T (+ bias)
   DeviceBuffer enc_pos_, dec_pos_;
   int64_t enc_positions_ = 0, dec_positions_ = 0;

@@ -1,4 +1,4 @@
-// attention_mma.cu — causal prefill attention on tensor cores for fp16/bf16 activations.
+// attention_mma.cu — causal prefill attention and encoder self-attention on tensor cores for fp16/bf16 activations.
 // Flash-attention style: a CTA owns 64 query rows of one (batch, head); 4 warps x 16 rows; K/V tiles of 64
 // keys are staged through shared memory with cp.async (double buffered) straight from the un-replicated GQA
 // cache [slot, Hkv, max_len, D]; S = Q K^T and O += P V run on mma.sync.m16n8k16 with fp32 accumulation and
@@ -25,11 +25,15 @@ using namespace mma;
 
 constexpr int kQTile = 64, kKTile = 64, kThreads = 128;
 
-template <typename T, int D>
+// kEncoder = false: causal prefill, K/V read from the cache [slot, Hkv, max_len, D] (`time` new rows after `offset`).
+// kEncoder = true: encoder self-attention (TransformerEncoder, src/layers/transformer.cc:427-471), K/V read from the fused
+// qkv rows [batch * time, 3d] themselves; non-causal, keys at or past lengths[b] masked (null = time).  Query tiles wholly
+// past the length are not computed: their rows are written as zeros (any finite value would do; they are ignored).
+template <typename T, int D, bool kEncoder>
 __global__ void __launch_bounds__(kThreads)
     attention_prefill_mma_kernel(const T* __restrict__ qkv, const T* __restrict__ k_cache, const T* __restrict__ v_cache,
-                                 int64_t time, int64_t offset, int H, int Hkv, int64_t max_len, float scale_log2,
-                                 T* __restrict__ out) {
+                                 const int32_t* __restrict__ lengths, int64_t time, int64_t offset, int H, int Hkv,
+                                 int64_t max_len, float scale_log2, T* __restrict__ out) {
   constexpr int LD = D + 8;                   // padded smem pitch (elements): conflict-free ldmatrix
   constexpr int CH = D / 8;                   // 16-byte chunks per row
   extern __shared__ __align__(16) uint8_t smem_raw[];
@@ -45,12 +49,31 @@ __global__ void __launch_bounds__(kThreads)
   const int kvh = h / (H / Hkv);
   const int64_t row_w = static_cast<int64_t>(H + 2 * Hkv) * D;
   const T* qbase = qkv + (b * time + q0) * row_w + static_cast<int64_t>(h) * D;
-  const T* kc = k_cache + (b * Hkv + kvh) * max_len * D;
-  const T* vc = v_cache + (b * Hkv + kvh) * max_len * D;
-
-  // keys visible to this query tile: 0 .. offset + min(q0+63, time-1)
-  const int64_t last_q = min(q0 + kQTile, time) - 1;
-  const int nkeys = static_cast<int>(offset + last_q + 1);
+  const T* kc;
+  const T* vc;
+  int64_t kv_w;                               // elements between consecutive keys
+  int nkeys;
+  if constexpr (kEncoder) {
+    nkeys = lengths ? lengths[b] : static_cast<int>(time);
+    if (q0 >= nkeys) {                        // every query row of the tile is past the length
+      for (int c = tid; c < kQTile * CH; c += kThreads) {
+        const int r = c / CH, ch = c % CH;
+        if (q0 + r < time)
+          *reinterpret_cast<uint4*>(out + ((b * time + q0 + r) * H + h) * D + ch * 8) = make_uint4(0u, 0u, 0u, 0u);
+      }
+      return;
+    }
+    kc = qkv + b * time * row_w + static_cast<int64_t>(H + kvh) * D;
+    vc = kc + static_cast<int64_t>(Hkv) * D;
+    kv_w = row_w;
+  } else {
+    // keys visible to this query tile: 0 .. offset + min(q0+63, time-1)
+    const int64_t last_q = min(q0 + kQTile, time) - 1;
+    nkeys = static_cast<int>(offset + last_q + 1);
+    kc = k_cache + (b * Hkv + kvh) * max_len * D;
+    vc = v_cache + (b * Hkv + kvh) * max_len * D;
+    kv_w = D;
+  }
   const int ntiles = (nkeys + kKTile - 1) / kKTile;
 
   auto load_kv = [&](int stage, int kt) {
@@ -58,7 +81,7 @@ __global__ void __launch_bounds__(kThreads)
     for (int c = tid; c < kKTile * CH; c += kThreads) {
       const int r = c / CH, ch = c % CH;
       const bool ok = k0 + r < nkeys;
-      const int64_t off = (ok ? k0 + r : 0) * D + ch * 8;
+      const int64_t off = (ok ? k0 + r : 0) * kv_w + ch * 8;
       cp16(sK + (stage * kKTile + r) * LD + ch * 8, kc + off, ok);
       cp16(sV + (stage * kKTile + r) * LD + ch * 8, vc + off, ok);
     }
@@ -116,7 +139,8 @@ __global__ void __launch_bounds__(kThreads)
       for (int r = 0; r < 4; ++r) {
         const int64_t key = kbase + j * 8 + 2 * t + (r & 1);
         const int64_t qp = qpos0 + (r >= 2 ? 8 : 0);
-        const float v = (key <= qp) ? s[j][r] * scale_log2 : -INFINITY;
+        const bool visible = kEncoder ? key < nkeys : key <= qp;
+        const float v = visible ? s[j][r] * scale_log2 : -INFINITY;
         s[j][r] = v;
         mx[r >> 1] = fmaxf(mx[r >> 1], v);
       }
@@ -406,11 +430,24 @@ template <typename T, int D>
 void launch_mma(const void* qkv, const void* kc, const void* vc, int64_t batch, int64_t time, int64_t offset, int H,
                 int Hkv, int64_t max_len, float scale, void* out, cudaStream_t st) {
   constexpr size_t smem = static_cast<size_t>(kQTile + 4 * kKTile) * (D + 8) * sizeof(T);
-  auto kernel = attention_prefill_mma_kernel<T, D>;
+  auto kernel = attention_prefill_mma_kernel<T, D, false>;
   allow_dynamic_smem(kernel, smem);
   dim3 grid(div_up(time, kQTile), H, static_cast<unsigned>(batch));
   kernel<<<grid, kThreads, smem, st>>>(static_cast<const T*>(qkv), static_cast<const T*>(kc), static_cast<const T*>(vc),
-                                       time, offset, H, Hkv, max_len, scale * 1.4426950408889634f, static_cast<T*>(out));
+                                       nullptr, time, offset, H, Hkv, max_len, scale * 1.4426950408889634f,
+                                       static_cast<T*>(out));
+  check_launch();
+}
+
+template <typename T, int D>
+void launch_encoder_mma(const void* qkv, const int32_t* lengths, int64_t batch, int S, int H, float scale, void* out,
+                        cudaStream_t st) {
+  constexpr size_t smem = static_cast<size_t>(kQTile + 4 * kKTile) * (D + 8) * sizeof(T);
+  auto kernel = attention_prefill_mma_kernel<T, D, true>;
+  allow_dynamic_smem(kernel, smem);
+  dim3 grid(div_up(S, kQTile), H, static_cast<unsigned>(batch));
+  kernel<<<grid, kThreads, smem, st>>>(static_cast<const T*>(qkv), nullptr, nullptr, lengths, S, 0, H, H, 0,
+                                       scale * 1.4426950408889634f, static_cast<T*>(out));
   check_launch();
 }
 
@@ -480,6 +517,21 @@ bool launch_attention_decode_mma(const void* qkv, void* kc, void* vc, const floa
   }
   return D == 128 ? launch_decode_mma_g<__nv_bfloat16, 128>(qkv, kc, vc, sn, cs, lens, batch, H, Hkv, max_len, interleave, scale, out, partials, tickets, splits, st)
                   : launch_decode_mma_g<__nv_bfloat16, 64>(qkv, kc, vc, sn, cs, lens, batch, H, Hkv, max_len, interleave, scale, out, partials, tickets, splits, st);
+}
+
+// tensor-core encoder self-attention; false = shape not covered (fp32, head_dim other than 64/128)
+bool launch_attention_encoder_mma(const void* qkv, const int32_t* lengths, int64_t batch, int S, int H, int D, float scale,
+                                  void* out, int dtype, cudaStream_t st) {
+  if (dtype == CT2B200_F32 || (D != 128 && D != 64)) return false;
+  if (batch * S == 0) return true;
+  if (dtype == CT2B200_F16) {
+    if (D == 128) launch_encoder_mma<__half, 128>(qkv, lengths, batch, S, H, scale, out, st);
+    else launch_encoder_mma<__half, 64>(qkv, lengths, batch, S, H, scale, out, st);
+  } else {
+    if (D == 128) launch_encoder_mma<__nv_bfloat16, 128>(qkv, lengths, batch, S, H, scale, out, st);
+    else launch_encoder_mma<__nv_bfloat16, 64>(qkv, lengths, batch, S, H, scale, out, st);
+  }
+  return true;
 }
 
 void launch_attention_prefill(const void* qkv, const void* kc, const void* vc, const int32_t* lengths, int64_t batch,

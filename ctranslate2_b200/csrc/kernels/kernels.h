@@ -143,6 +143,9 @@ void launch_attention_prefill_simple(const void* qkv, const void* kc, const void
 bool launch_attention_prefill_mma(const void* qkv, const void* kc, const void* vc, int64_t batch, int64_t time,
                                   int64_t offset, int H, int Hkv, int D, int64_t max_len, float scale, void* out,
                                   int dtype, cudaStream_t st);
+// encoder self-attention of launch_attention_encoder on tensor cores (fp16 / bf16, head_dim 64 or 128); false = not covered
+bool launch_attention_encoder_mma(const void* qkv, const int32_t* lengths, int64_t batch, int S, int H, int D, float scale,
+                                  void* out, int dtype, cudaStream_t st);
 // attention_decode.cu — persistent work-balanced decode attention; false = shape not covered
 bool launch_attention_decode_persistent(const void* qkv, void* kc, void* vc, const float* sn, const float* cs,
                                         const int32_t* lens, int64_t batch, int H, int Hkv, int D, int64_t max_len,
@@ -171,7 +174,8 @@ void launch_mul_inplace(void* a_inout, const void* b, int64_t n, int dtype, cuda
 // seq2seq.cu — encoder-decoder path (Translator): embeddings + positions, LayerNorm, head_dim-agnostic attention, beam search
 void launch_embed_pos(const void* w, const float* w_scale, const int32_t* ids, int64_t rows, int64_t depth, float emb_scale,
                       const void* pos, int64_t time, const int32_t* step_ptr, bool zero_first, void* y, int dtype,
-                      cudaStream_t st);
+                      cudaStream_t st, const void* w2 = nullptr, const float* w2_scale = nullptr,
+                      const int32_t* ids2 = nullptr);
 void launch_layer_norm(const void* x, const void* gamma, const void* beta, int64_t rows, int64_t cols, float eps, void* y,
                        int8_t* q, float* scale, bool round, int dtype, cudaStream_t st);
 void launch_attention_encoder(const void* qkv, const int32_t* lengths, int64_t batch, int S, int H, int D, float scale,

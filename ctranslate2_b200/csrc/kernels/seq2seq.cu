@@ -26,12 +26,15 @@ template <> __device__ __forceinline__ float lowest_of<__nv_bfloat16>() { return
 // ---------------------------------------------------------------------------------------------
 // layers::Embeddings (+ int8 dequantization, common.cc:64-81) * embeddings scale (transformer.cc:382-402, ops::Mul in T)
 // + PositionEncoder (common.cc:170-229, ops::Add in T).  Row r of [batch, time]: position = r % time, or *step_ptr for the
-// single-token decoder step (device-resident so that the step is CUDA-graph capturable).
+// single-token decoder step (device-resident so that the step is CUDA-graph capturable).  w2 (optional): a second table
+// (token types) looked up with ids2 and merged by ADD in T before the scale (ParallelEmbeddings, common.cc:116-148).
 // ---------------------------------------------------------------------------------------------
 template <typename T>
 __global__ void embed_pos_kernel(const void* __restrict__ w, const float* __restrict__ w_scale, const int32_t* __restrict__ ids,
                                  int64_t depth, float emb_scale, const T* __restrict__ pos, int64_t time,
-                                 const int32_t* __restrict__ step_ptr, bool zero_first, T* __restrict__ y) {
+                                 const int32_t* __restrict__ step_ptr, bool zero_first, T* __restrict__ y,
+                                 const void* __restrict__ w2, const float* __restrict__ w2_scale,
+                                 const int32_t* __restrict__ ids2) {
   griddep_launch();
   griddep_wait();
   const int64_t r = blockIdx.x;
@@ -44,6 +47,12 @@ __global__ void embed_pos_kernel(const void* __restrict__ w, const float* __rest
     if (zero) v = 0.f;
     else if (w_scale) v = round_to<T>(__fdiv_rn(static_cast<float>(static_cast<const int8_t*>(w)[id * depth + j]), w_scale[id]));
     else v = to_f32(static_cast<const T*>(w)[id * depth + j]);
+    if (w2) {
+      const int64_t id2 = ids2[r];
+      const float v2 = w2_scale ? round_to<T>(__fdiv_rn(static_cast<float>(static_cast<const int8_t*>(w2)[id2 * depth + j]), w2_scale[id2]))
+                                : to_f32(static_cast<const T*>(w2)[id2 * depth + j]);
+      v = round_to<T>(v2 + v);
+    }
     if (emb_scale != 0.f && !zero) v = round_to<T>(v * es);
     if (pos) v = round_to<T>(v + to_f32(pos[t * depth + j]));
     y[r * depth + j] = from_f32<T>(v);
@@ -939,10 +948,11 @@ __global__ void __launch_bounds__(256) gemm_f32_kernel(const float* __restrict__
 // ---------------------------------------------------------------------------------------------
 void launch_embed_pos(const void* w, const float* w_scale, const int32_t* ids, int64_t rows, int64_t depth, float emb_scale,
                       const void* pos, int64_t time, const int32_t* step_ptr, bool zero_first, void* y, int dtype,
-                      cudaStream_t st) {
+                      cudaStream_t st, const void* w2, const float* w2_scale, const int32_t* ids2) {
   if (rows == 0) return;
   CT2_DISPATCH_DTYPE(dtype, (launch_pdl(embed_pos_kernel<T>, dim3(rows), dim3(128), 0, st, w, w_scale, ids, depth, emb_scale,
-                                        static_cast<const T*>(pos), time, step_ptr, zero_first, static_cast<T*>(y))));
+                                        static_cast<const T*>(pos), time, step_ptr, zero_first, static_cast<T*>(y), w2,
+                                        w2_scale, ids2)));
   check_launch();
 }
 

@@ -373,6 +373,19 @@ def attention_encoder(qkv, num_heads, head_dim, batch, lengths=None, scale=None)
     return out
 
 
+def attention_encoder_mma(qkv, num_heads, head_dim, batch, lengths=None, scale=None):
+    """attention_encoder on tensor cores (fp16 / bf16, head_dim 64 or 128; ValueError otherwise).  Rows past a length are
+    unspecified but finite."""
+    qkv = _rows(qkv)
+    d = num_heads * head_dim
+    S = qkv.shape[0] // batch if batch else 0
+    scale = head_dim ** -0.5 if scale is None else scale
+    out = torch.empty((batch * S, d), dtype=qkv.dtype, device=qkv.device)
+    check(lib().ct2b200_attention_encoder_mma(_p(qkv), _p(lengths), ctypes.c_int64(batch), S, num_heads, head_dim,
+                                              ctypes.c_float(scale), _p(out), _dt(qkv), _stream()))
+    return out
+
+
 def attention_causal(qkv, num_heads, head_dim, batch, scale=None):
     """Teacher-forced causal self-attention: qkv [batch * time, 3d] -> out [batch * time, d]."""
     qkv = _rows(qkv)

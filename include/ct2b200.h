@@ -219,6 +219,13 @@ CT2B200_API int ct2b200_attention_prefill(const void* qkv_d, void* k_cache_d, vo
  * (NULL = S; a length of 0 gives a zero row).  out_d [batch * S, d]. */
 CT2B200_API int ct2b200_attention_encoder(const void* qkv_d, const int32_t* lengths_d, int64_t batch, int S, int H, int D,
                                           float scale, void* out_d, int dtype, void* stream);
+/* The same encoder self-attention on tensor cores (the kernel of encoder-only models, ct2b200_encoder_open): mma.sync
+ * m16n8k16 tiles of 64 queries x 64 keys, fp32 online softmax, P rounded to T before P.V (flash-attention style instead of
+ * the reference's MatMul + SoftMax + MatMul, src/layers/attention.cc:178-287).  fp16 / bf16 and head_dim 64 or 128 only
+ * ("invalid argument" otherwise).  Key tiles past lengths_d[b] are not read; query tiles wholly past it are written as zeros,
+ * the other rows past it attend like the valid ones. */
+CT2B200_API int ct2b200_attention_encoder_mma(const void* qkv_d, const int32_t* lengths_d, int64_t batch, int S, int H, int D,
+                                              float scale, void* out_d, int dtype, void* stream);
 /* Teacher-forced causal decoder self-attention: qkv_d [batch * time, 3d]; row (b, t) attends to rows (b, j), j <= t.
  * out_d [batch * time, d]. */
 CT2B200_API int ct2b200_attention_causal(const void* qkv_d, int64_t batch, int time, int H, int D, float scale, void* out_d,
@@ -502,6 +509,32 @@ CT2B200_API int ct2b200_whisper_detect_language(ct2b200_translator* t, const flo
 /* Host only (no device): negative_dtw + backtrace (src/dtw.cc), the function whisper_align runs on its matrices.
  * x_h [n, m] f32; out_path_h [n + m, 2] (row, column) pairs, out_len_h = their count. */
 CT2B200_API int ct2b200_negative_dtw_host(const float* x_h, int64_t n, int64_t m, int32_t* out_path_h, int32_t* out_len_h);
+
+/* ---------------------------------------------------------------------------------------------
+ * Encoder-only models: ctranslate2::Encoder — python/cpp/encoder.cc (forward_batch), models::EncoderReplica::forward_impl
+ * (src/models/language_model.cc:302-400), TransformerEncoder (src/layers/transformer.cc:405-471).  Serves
+ * TransformerEncoderSpec directories (BERT, DistilBERT, RoBERTa, XLM-R class): one token table or tokens + token types merged
+ * by ADD, stored position encodings, optional layernorm_embedding, pre- or post-norm LayerNorm layers with ReLU / GELU /
+ * GELUTanh, optional final norm, optional pooler_dense + pooler_activation on the first position.  Every other feature the
+ * spec can hold is refused at open.  ct2b200_generator_config: device / compute_type / weight_type are honoured, the rest is
+ * ignored (arenas grow on demand).  fp16 / bf16 compute with head_dim 64 or 128 runs ct2b200_attention_encoder_mma.
+ * ------------------------------------------------------------------------------------------- */
+typedef struct ct2b200_encoder ct2b200_encoder;
+CT2B200_API ct2b200_encoder* ct2b200_encoder_open(const char* model_dir, const ct2b200_generator_config* config);
+CT2B200_API void ct2b200_encoder_close(ct2b200_encoder* e);
+/* Host only: the geometry parse_encoder_config reads from `model_dir`, as JSON (refuses what the engine cannot run). */
+CT2B200_API int ct2b200_encoder_summary(const char* model_dir, char* json_out, size_t capacity);
+/* Encoder::forward_batch on ids.  HOST buffers: ids_h [batch, max_length] int32 right-padded, lengths_h [batch] in
+ * [1, max_length], token_type_ids_h [batch, max_length] or NULL (zeros, the reference's placeholder); max_length <= the
+ * position table.  last_hidden_state_h [batch, max_length, d_model] f32 (positions past a row's length are unspecified);
+ * pooler_output_h [batch, d_model] f32 or NULL (models with a pooler). */
+CT2B200_API int ct2b200_encoder_forward(ct2b200_encoder* e, const int32_t* ids_h, const int32_t* lengths_h,
+                                        const int32_t* token_type_ids_h, int64_t batch, int64_t max_length,
+                                        float* last_hidden_state_h, float* pooler_output_h);
+/* Device-timed encoder passes on resident synthetic ids of lengths_h [batch] (<= max_length): median_ms = the median of
+ * `iters` passes after `warmup` untimed ones. */
+CT2B200_API int ct2b200_encoder_bench(ct2b200_encoder* e, const int32_t* lengths_h, int64_t batch, int64_t max_length,
+                                      int64_t iters, int64_t warmup, float* median_ms);
 
 #ifdef __cplusplus
 }

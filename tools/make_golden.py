@@ -539,8 +539,77 @@ def make_whisper_sampling_fixture():
     print("whisper sampling fixture:", len(fixture["cases"]), "cases")
 
 
+ENCODER_VARIANTS = {
+    # BERT-like: tokens + token types, learned positions, layernorm_embedding, post-norm GELU, pooler
+    "tiny_encoder": {},
+    "tiny_encoder_prenorm": {"pre_norm": True, "activation": 0, "type_vocab_size": 0, "layernorm_embedding": False},
+    "tiny_encoder_nopooler": {"pooler": False, "activation": 1},
+}
+
+
+def _ref_encoder(model_dir, compute, ids, types):
+    """Encoder::forward_batch of the unmodified reference (CPU) through tools/ref_encoder.cc, built by tools/ref_encoder.mk
+    against oracle/_ref/libct2ref.so into a temporary directory: per row, (hidden [len, d], pooled [d] or None)."""
+    import subprocess
+    import tempfile
+    out_dir = os.path.join(tempfile.gettempdir(), "ct2ref_encoder")
+    subprocess.run(["make", "-s", "-f", "tools/ref_encoder.mk", "encoder", "ENCODER_OUT=" + out_dir], cwd=ROOT, check=True)
+    lines = ["%s\t%s" % (model_dir, compute)]
+    for b, row in enumerate(ids):
+        lines.append(" ".join(map(str, row)) + "\t" + (" ".join(map(str, types[b])) if types is not None else ""))
+    r = subprocess.run([os.path.join(out_dir, "ref_encoder")], input="\n".join(lines) + "\n", capture_output=True, text=True,
+                       check=True)
+    res = []
+    for line in r.stdout.rstrip("\n").split("\n"):
+        h, p = line.split("\t")
+        res.append(([float(x) for x in h.split(" ")], [float(x) for x in p.split(" ")] if p else None))
+    return res
+
+
+def make_encoder_fixture():
+    """tests/golden/tiny_encoder*/ (synthetic TransformerEncoderSpec models, int8 storage, d 64 = 1 head of 64, 16 positions)
+    and tests/golden/encoder_ref.npz: the reference's Encoder::forward_batch (CPU build) in float32 and int8 on ragged
+    batches with a 1-token row and a row that fills the position table, with and without token types.  Case k is stored as
+    c<k>_model, c<k>_compute, c<k>_ids [B, T] (right-padded), c<k>_lens [B], c<k>_types [B, T] (when given), c<k>_hidden
+    [sum(lens), d] (the valid positions, row after row) and c<k>_pooled [B, d] (models with a pooler)."""
+    from ctranslate2_b200.converters.synthetic import EncoderConfig, write_encoder_model
+    rng = np.random.default_rng(2024)
+    arrays, k = {}, 0
+    for m, (name, kw) in enumerate(ENCODER_VARIANTS.items()):
+        cfg = EncoderConfig(num_layers=2, num_heads=1, d_model=64, ffn_dim=128, vocab_size=50, max_positions=16,
+                            layer_norm_epsilon=1e-12, **kw)
+        path = os.path.join(OUT, name)
+        write_encoder_model(path, cfg, "int8", seed=11 + m)
+        for compute in ("float32", "int8"):
+            for with_types in ((False, True) if cfg.type_vocab_size else (False,)):
+                if compute == "int8" and not with_types and cfg.type_vocab_size:
+                    continue
+                lens = np.array([16, 1, 7], np.int32)
+                ids = np.zeros((len(lens), lens.max()), np.int32)
+                types = np.zeros_like(ids) if with_types else None
+                for b, n in enumerate(lens):
+                    ids[b, :n] = rng.integers(0, cfg.vocab_size, n)
+                    if with_types:
+                        types[b, :n] = rng.integers(0, cfg.type_vocab_size, n)
+                res = _ref_encoder(os.path.abspath(path), compute, [ids[b, :n].tolist() for b, n in enumerate(lens)],
+                                   None if types is None else [types[b, :n].tolist() for b, n in enumerate(lens)])
+                c = "c%d_" % k
+                arrays.update({c + "model": np.array(name), c + "compute": np.array(compute), c + "ids": ids, c + "lens": lens,
+                               c + "hidden": np.array([v for h, _ in res for v in h], np.float32).reshape(-1, cfg.d_model)})
+                if types is not None:
+                    arrays[c + "types"] = types
+                if res[0][1] is not None:
+                    arrays[c + "pooled"] = np.array([p for _, p in res], np.float32)
+                k += 1
+    np.savez_compressed(os.path.join(OUT, "encoder_ref.npz"), **arrays)
+    print("encoder fixture:", k, "cases")
+
+
 def main():
     os.makedirs(OUT, exist_ok=True)
+    if "--encoder-only" in sys.argv:
+        make_encoder_fixture()
+        return
     if "--whisper-sampling-only" in sys.argv:
         make_whisper_sampling_fixture()
         return
@@ -640,6 +709,7 @@ def main():
     make_whisper_fixture()
     make_whisper_align_fixture()
     make_whisper_sampling_fixture()
+    make_encoder_fixture()
     print("done")
 
 
