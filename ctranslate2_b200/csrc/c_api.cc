@@ -144,14 +144,6 @@ CT2B200_API int ct2b200_dense_s8_glu(const int8_t* xq, const float* x_scale, con
   });
 }
 
-namespace {
-void rows_to_int8(const void* x, const void* gamma, float eps, int64_t m, int64_t k, int dtype, int8_t* xq, float* xs,
-                  cudaStream_t st) {
-  if (gamma) launch_rms_norm(gamma, x, m, k, eps, false, nullptr, xq, xs, dtype, st);
-  else launch_quantize_rows(x, dtype, m, k, true, xq, xs, st);
-}
-}  // namespace
-
 CT2B200_API int ct2b200_dense_s8_rows(const void* x, const void* gamma, float eps, const int8_t* w, const float* w_scale,
                           const void* bias, const void* residual, int act, int64_t m, int64_t n, int64_t k, void* y,
                           int dtype, int8_t* xq, float* x_scale, void* stream) {

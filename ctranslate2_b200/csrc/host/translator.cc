@@ -199,22 +199,9 @@ Seq2SeqConfig parse_encoder_config(const ModelFile& f) {
 // =============================================================================================
 // loading
 // =============================================================================================
-void Translator::load_dense(const ModelFile& f, const std::string& prefix, DenseWeights& w) {
-  const bool int8 = load_dense_matrix(f, prefix, dtype_, weight_type_, stream_, w.weight, w.scale, w.n, w.k);
-  w.kind = int8 ? DenseWeights::INT8 : DenseWeights::FLOAT16;
-  CT2_REQUIRE(!int8 || w.k % 16 == 0, "int8 Dense layers need an input size that is a multiple of 16");
-  mc_.weight_bytes += w.weight.bytes + w.scale.bytes;
-  if (const HostVariable* b = f.find(prefix + "/bias")) {
-    const auto bytes = convert_to_dtype(*b, dtype_);
-    upload(w.bias, bytes.data(), bytes.size());
-  }
-}
-
 void Translator::load_norm(const ModelFile& f, const std::string& prefix, NormWeights& n) {
-  const auto g = convert_to_dtype(f.get(prefix + "/gamma"), dtype_);
-  const auto b = convert_to_dtype(f.get(prefix + "/beta"), dtype_);
-  upload(n.gamma, g.data(), g.size());
-  upload(n.beta, b.data(), b.size());
+  upload_as(n.gamma, f.get(prefix + "/gamma"), dtype_);
+  upload_as(n.beta, f.get(prefix + "/beta"), dtype_);
 }
 
 namespace {
@@ -234,27 +221,25 @@ std::vector<float> sinusoidal_positions(int64_t max_time, int64_t depth) {
 }
 }  // namespace
 
-Translator::Translator(const std::string& model_dir, const ct2b200_generator_config& cfg, bool encoder_only) {
-  device_ = cfg.device;
-  CT2_CUDA_CHECK(cudaSetDevice(device_));
-  int major = 0;
-  CT2_CUDA_CHECK(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, device_));
-  if (major != 9)
-    throw std::runtime_error("ct2b200 is built for sm_90a (H100); found compute capability major " + std::to_string(major));
-  CT2_CUDA_CHECK(cudaDeviceGetAttribute(&sm_count_, cudaDevAttrMultiProcessorCount, device_));
-  CT2_CUDA_CHECK(cudaStreamCreateWithFlags(&stream_, cudaStreamNonBlocking));
+Translator::Translator(const std::string& model_dir, const ct2b200_generator_config& cfg, bool encoder_only)
+    : gpu_(cfg.device) {
   dtype_ = cfg.compute_type;
-  weight_type_ = cfg.weight_type;
   use_graph_ = cfg.use_cuda_graph != 0;
   CT2_REQUIRE(cfg.tp_size <= 1, "the Translator engine does not run tensor parallel");
 
   ModelFile f(model_dir);
   mc_ = encoder_only ? parse_encoder_config(f) : parse_seq2seq_config(f);
+  // no AWQ arm here: AWQ weights are refused as an unsupported weight type
+  const DenseLoad opt{dtype_, cfg.weight_type, stream()};
+  auto load = [&](const std::string& prefix, DenseWeights& w) {
+    mc_.weight_bytes += load_dense(f, prefix, opt, w);
+    CT2_REQUIRE(w.kind != DenseWeights::INT8 || w.k % 16 == 0, "int8 Dense layers need an input size that is a multiple of 16");
+  };
   if (mc_.encoder_only) {
-    load_dense(f, f.find("encoder/embeddings_0/weight") ? "encoder/embeddings_0" : "encoder/embeddings", enc_emb_);
-    if (mc_.type_vocab) load_dense(f, "encoder/embeddings_1", type_emb_);
+    load(f.find("encoder/embeddings_0/weight") ? "encoder/embeddings_0" : "encoder/embeddings", enc_emb_);
+    if (mc_.type_vocab) load("encoder/embeddings_1", type_emb_);
     if (mc_.has_emb_norm) load_norm(f, "encoder/layernorm_embedding", emb_norm_);
-    if (mc_.has_pooler) load_dense(f, "pooler_dense", pooler_);
+    if (mc_.has_pooler) load("pooler_dense", pooler_);
   } else if (mc_.whisper) {
     // the convolutions run as im2col + float Dense: weights [d, Cin, 3] flattened to [d, Cin * 3] in T (the reference keeps
     // them in float on CUDA too, model.cc:204-223; an int8-stored convolution is dequantized here: w = q / scale)
@@ -276,26 +261,21 @@ Translator::Translator(const std::string& model_dir, const ct2b200_generator_con
         flat.data = reinterpret_cast<const uint8_t*>(deq.data());
         flat.nbytes = deq.size() * 4;
       }
-      const auto bytes = convert_to_dtype(flat, dtype_);
-      upload(w.weight, bytes.data(), bytes.size());
+      mc_.weight_bytes += upload_as(w.weight, flat, dtype_);
       w.kind = DenseWeights::FLOAT16;
       w.n = wt.shape[0];
       w.k = wt.shape[1] * wt.shape[2];
-      mc_.weight_bytes += bytes.size();
-      if (const HostVariable* b = f.find(prefix + "/bias")) {
-        const auto bb = convert_to_dtype(*b, dtype_);
-        upload(w.bias, bb.data(), bb.size());
-      }
+      if (const HostVariable* b = f.find(prefix + "/bias")) upload_as(w.bias, *b, dtype_);
     };
     CT2_REQUIRE(dtype_ == CT2B200_F32 || (mc_.n_mels * 3) % 8 == 0, "n_mels * 3 must be a multiple of 8 for float16 / bfloat16");
     load_conv("encoder/conv1", conv1_);
     load_conv("encoder/conv2", conv2_);
   } else {
-    load_dense(f, embeddings_scope(f, "encoder"), enc_emb_);
+    load(embeddings_scope(f, "encoder"), enc_emb_);
   }
   if (!mc_.encoder_only) {
-    load_dense(f, "decoder/embeddings", dec_emb_);
-    load_dense(f, "decoder/projection", projection_);
+    load("decoder/embeddings", dec_emb_);
+    load("decoder/projection", projection_);
   }
   if (mc_.has_enc_final_norm) load_norm(f, "encoder/layer_norm", enc_norm_);
   if (mc_.has_dec_final_norm) load_norm(f, "decoder/layer_norm", dec_norm_);
@@ -303,31 +283,30 @@ Translator::Translator(const std::string& model_dir, const ct2b200_generator_con
   for (int l = 0; l < mc_.enc_layers; ++l) {
     const std::string p = "encoder/layer_" + std::to_string(l) + "/";
     load_norm(f, p + "self_attention/layer_norm", enc_[l].self.norm);
-    load_dense(f, p + "self_attention/linear_0", enc_[l].self.in);
-    load_dense(f, p + "self_attention/linear_1", enc_[l].self.out);
+    load(p + "self_attention/linear_0", enc_[l].self.in);
+    load(p + "self_attention/linear_1", enc_[l].self.out);
     load_norm(f, p + "ffn/layer_norm", enc_[l].ffn.norm);
-    load_dense(f, p + "ffn/linear_0", enc_[l].ffn.ff1);
-    load_dense(f, p + "ffn/linear_1", enc_[l].ffn.ff2);
+    load(p + "ffn/linear_0", enc_[l].ffn.ff1);
+    load(p + "ffn/linear_1", enc_[l].ffn.ff2);
   }
   dec_.resize(mc_.dec_layers);
   for (int l = 0; l < mc_.dec_layers; ++l) {
     const std::string p = "decoder/layer_" + std::to_string(l) + "/";
     load_norm(f, p + "self_attention/layer_norm", dec_[l].self.norm);
-    load_dense(f, p + "self_attention/linear_0", dec_[l].self.in);
-    load_dense(f, p + "self_attention/linear_1", dec_[l].self.out);
+    load(p + "self_attention/linear_0", dec_[l].self.in);
+    load(p + "self_attention/linear_1", dec_[l].self.out);
     load_norm(f, p + "attention/layer_norm", dec_[l].cross.norm);
-    load_dense(f, p + "attention/linear_0", dec_[l].cross.in);
-    load_dense(f, p + "attention/linear_1", dec_[l].cross.kv);
-    load_dense(f, p + "attention/linear_2", dec_[l].cross.out);
+    load(p + "attention/linear_0", dec_[l].cross.in);
+    load(p + "attention/linear_1", dec_[l].cross.kv);
+    load(p + "attention/linear_2", dec_[l].cross.out);
     load_norm(f, p + "ffn/layer_norm", dec_[l].ffn.norm);
-    load_dense(f, p + "ffn/linear_0", dec_[l].ffn.ff1);
-    load_dense(f, p + "ffn/linear_1", dec_[l].ffn.ff2);
+    load(p + "ffn/linear_0", dec_[l].ffn.ff1);
+    load(p + "ffn/linear_1", dec_[l].ffn.ff2);
   }
   // position encodings: stored table (PositionEmbedding) or sinusoidal (SinusoidalPositionEncoder, 500 positions or more)
   auto load_positions = [&](const std::string& scope, DeviceBuffer& dst) -> int64_t {
     if (const HostVariable* e = f.find(scope + "/position_encodings/encodings")) {
-      const auto bytes = convert_to_dtype(*e, dtype_);
-      upload(dst, bytes.data(), bytes.size());
+      upload_as(dst, *e, dtype_);
       return e->shape[0];
     }
     const int64_t count = std::max<int64_t>(500, cfg.max_length);
@@ -337,27 +316,20 @@ Translator::Translator(const std::string& model_dir, const ct2b200_generator_con
     v.type_id = 0;
     v.data = reinterpret_cast<const uint8_t*>(enc.data());
     v.nbytes = enc.size() * 4;
-    const auto bytes = convert_to_dtype(v, dtype_);
-    upload(dst, bytes.data(), bytes.size());
+    upload_as(dst, v, dtype_);
     return count;
   };
   enc_positions_ = load_positions("encoder", enc_pos_);
   if (!mc_.encoder_only) dec_positions_ = load_positions("decoder", dec_pos_);
-  SplitKWorkspace::get(stream_);   // create the split-K scratch outside any graph capture
   CT2_CUDA_CHECK(cudaDeviceSynchronize());
 }
 
 Translator::~Translator() {
   if (host_pinned_) cudaFreeHost(host_pinned_);
-  if (stream_) {
-    cudaStreamSynchronize(stream_);
-    SplitKWorkspace::release(stream_);
-    cudaStreamDestroy(stream_);
-  }
 }
 
 void Translator::drop_graph() {
-  CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));
+  CT2_CUDA_CHECK(cudaStreamSynchronize(stream()));
   graph_.reset();
 }
 
@@ -435,26 +407,21 @@ void Translator::ensure_rows(int64_t entries, int64_t enc_rows, int64_t rows) {
 // =============================================================================================
 void Translator::dense(const DenseWeights& w, const NormWeights* pre, const void* x, int64_t rows, const void* residual,
                        int act, void* y, bool prequantized, int64_t ldy) {
-  if (ldy == 0) ldy = w.n;
+  const void* src = x;
   if (w.kind == DenseWeights::INT8) {
     if (prequantized)
       ;                                            // the post-norm kernel before this call left Quantize(x) in xq_ / xs_
     else if (pre)
       launch_layer_norm(x, pre->gamma.ptr, pre->beta.ptr, rows, w.k, mc_.eps, nullptr, xq_.as<int8_t>(), xs_.as<float>(),
-                        mc_.round_before_cast, dtype_, stream_);
+                        mc_.round_before_cast, dtype_, stream());
     else
-      launch_quantize_rows(x, dtype_, rows, w.k, mc_.round_before_cast, xq_.as<int8_t>(), xs_.as<float>(), stream_);
-    DenseEpilogue e{xs_.as<float>(), w.scale.as<float>(), w.bias.ptr, residual, y, nullptr, act, ldy};
-    gemm_s8(xq_.as<int8_t>(), w.weight.as<int8_t>(), rows, w.n, w.k, e, dtype_, CT2B200_GEMM_AUTO, stream_);
-  } else {
-    const void* src = x;
-    if (pre) {
-      launch_layer_norm(x, pre->gamma.ptr, pre->beta.ptr, rows, w.k, mc_.eps, xn_.ptr, nullptr, nullptr, true, dtype_, stream_);
-      src = xn_.ptr;
-    }
-    CT2_REQUIRE(ldy == w.n, "float Dense writes contiguous rows");
-    gemm_float(src, w.weight.ptr, w.bias.ptr, residual, act, rows, w.n, w.k, y, dtype_, stream_);
+      launch_quantize_rows(x, dtype_, rows, w.k, mc_.round_before_cast, xq_.as<int8_t>(), xs_.as<float>(), stream());
+  } else if (pre) {
+    launch_layer_norm(x, pre->gamma.ptr, pre->beta.ptr, rows, w.k, mc_.eps, xn_.ptr, nullptr, nullptr, true, dtype_, stream());
+    src = xn_.ptr;
   }
+  dense_forward(w, xq_.as<int8_t>(), xs_.as<float>(), src, rows, residual, act, y, ldy, dtype_, CT2B200_GEMM_AUTO, nullptr,
+                stream());
 }
 
 // Row stride of the logits for a search: INT8 projections write rows padded to a multiple of 8 elements (16-byte stores in the
@@ -472,7 +439,7 @@ void Translator::set_logits_ld(BeamState& bs) {
 bool Translator::post_norm(const NormWeights& n, void* x, int64_t rows, const DenseWeights* next) {
   const bool q = next && next->kind == DenseWeights::INT8 && next->k == mc_.d_model;
   launch_layer_norm(x, n.gamma.ptr, n.beta.ptr, rows, mc_.d_model, mc_.eps, x, q ? xq_.as<int8_t>() : nullptr,
-                    q ? xs_.as<float>() : nullptr, q ? mc_.round_before_cast : true, dtype_, stream_);
+                    q ? xs_.as<float>() : nullptr, q ? mc_.round_before_cast : true, dtype_, stream());
   return q;
 }
 
@@ -480,7 +447,7 @@ bool Translator::post_norm(const NormWeights& n, void* x, int64_t rows, const De
 void Translator::run_encoder(int64_t batch, int64_t S) {
   launch_embed_pos(enc_emb_.weight.ptr, enc_emb_.kind == DenseWeights::INT8 ? enc_emb_.scale.as<float>() : nullptr,
                    src_ids_.as<int32_t>(), batch * S, mc_.d_model, mc_.enc_emb_scale, enc_pos_.ptr, S, nullptr, false, x_.ptr,
-                   dtype_, stream_);
+                   dtype_, stream());
   run_encoder_layers(batch, S, src_lens_.as<int32_t>());
 }
 
@@ -496,9 +463,9 @@ void Translator::run_encoder_layers(int64_t batch, int64_t S, const int32_t* len
     // encoder-only models run the tensor-core kernel where it covers the shape; the Translator and Whisper encoders keep
     // the generic one
     if (!mc_.encoder_only || !launch_attention_encoder_mma(qkv_.ptr, lens_d, batch, static_cast<int>(S), mc_.num_heads,
-                                                           mc_.head_dim, scale, ctx_.ptr, dtype_, stream_))
+                                                           mc_.head_dim, scale, ctx_.ptr, dtype_, stream()))
       launch_attention_encoder(qkv_.ptr, lens_d, batch, static_cast<int>(S), mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, dtype_,
-                               stream_);
+                               stream());
     dense(w.self.out, nullptr, ctx_.ptr, rows, x_.ptr, -1, x_.ptr);
     xq = !pre && post_norm(w.self.norm, x_.ptr, rows, &w.ffn.ff1);
     dense(w.ffn.ff1, pre ? &w.ffn.norm : nullptr, x_.ptr, rows, nullptr, mc_.enc_activation, h_.ptr, xq);
@@ -507,9 +474,9 @@ void Translator::run_encoder_layers(int64_t batch, int64_t S, const int32_t* len
   }
   if (mc_.has_enc_final_norm)
     launch_layer_norm(x_.ptr, enc_norm_.gamma.ptr, enc_norm_.beta.ptr, rows, d, mc_.eps, memory_.ptr, nullptr, nullptr, true, dtype_,
-                      stream_);
+                      stream());
   else
-    CT2_CUDA_CHECK(cudaMemcpyAsync(memory_.ptr, x_.ptr, rows * d * dtype_size(dtype_), cudaMemcpyDeviceToDevice, stream_));
+    CT2_CUDA_CHECK(cudaMemcpyAsync(memory_.ptr, x_.ptr, rows * d * dtype_size(dtype_), cudaMemcpyDeviceToDevice, stream()));
 }
 
 // the memory keys / values of every decoder layer, once per batch (cached_attn_keys / values, attention.cc:385-428)
@@ -534,10 +501,10 @@ bool Translator::run_decoder_layers(int64_t rows, int rows_per_entry, int64_t S,
     dense(w.cross.in, pre ? &w.cross.norm : nullptr, x_.ptr, rows, nullptr, -1, q_.ptr, xq);
     if (capture && (*capture)[l].masks)
       launch_attention_cross_capture(q_.ptr, mem_kv_[l].ptr, src_lens_.as<int32_t>(), rows, rows_per_entry, static_cast<int>(S),
-                                     mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, (*capture)[l], dtype_, stream_);
+                                     mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, (*capture)[l], dtype_, stream());
     else
       launch_attention_cross(q_.ptr, mem_kv_[l].ptr, src_lens_.as<int32_t>(), rows, rows_per_entry, static_cast<int>(S),
-                             mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, dtype_, stream_);
+                             mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, dtype_, stream());
     dense(w.cross.out, nullptr, ctx_.ptr, rows, x_.ptr, -1, x_.ptr);
     xq = !pre && post_norm(w.cross.norm, x_.ptr, rows, &w.ffn.ff1);
     dense(w.ffn.ff1, pre ? &w.ffn.norm : nullptr, x_.ptr, rows, nullptr, mc_.dec_activation, h_.ptr, xq);
@@ -552,7 +519,7 @@ bool Translator::run_decoder_layers(int64_t rows, int rows_per_entry, int64_t S,
 void Translator::embed_decoder(const int32_t* ids_d, int64_t rows, int64_t time, const int32_t* step_ptr) {
   launch_embed_pos(dec_emb_.weight.ptr, dec_emb_.kind == DenseWeights::INT8 ? dec_emb_.scale.as<float>() : nullptr, ids_d, rows,
                    mc_.d_model, mc_.dec_emb_scale, dec_pos_.ptr, time, step_ptr, mc_.start_from_zero_embedding, x_.ptr, dtype_,
-                   stream_);
+                   stream());
 }
 
 // TransformerDecoder::decode for one target position of every beam row (transformer.cc:621-871)
@@ -563,7 +530,7 @@ void Translator::decoder_step(int64_t rows, int beam, int64_t batch, int64_t S) 
   embed_decoder(beam_.next_ids.as<int32_t>(), rows, 1, step_ptr);
   const bool xq = run_decoder_layers(rows, beam, S, [&](int l) {
     launch_attention_beam_self(qkv_.ptr, self_k_[l].ptr, self_v_[l].ptr, beam_.anc.as<int32_t>(), step_ptr, rows,
-                               static_cast<int>(cap_steps_), mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, dtype_, stream_);
+                               static_cast<int>(cap_steps_), mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, dtype_, stream());
   });
   dense(projection_, mc_.has_dec_final_norm ? &dec_norm_ : nullptr, x_.ptr, rows, nullptr, -1, logits_.ptr, xq, logits_ld_);
 }
@@ -573,16 +540,16 @@ void Translator::launch_or_capture_step(const BeamState& bs, int64_t S, const st
   auto step = [&] {
     decoder_step(rows, bs.beam, bs.batch, S);
     if (bs.sample_topk >= 0)
-      beam_.sample_step(logits_.ptr, bs, dtype_, stream_);
+      beam_.sample_step(logits_.ptr, bs, dtype_, stream());
     else
-      beam_.step(logits_.ptr, bs, dtype_, stream_);
+      beam_.step(logits_.ptr, bs, dtype_, stream());
   };
   if (!use_graph_) {
     step();
     return;
   }
-  graph_.capture(stream_, key, step);
-  graph_.launch(stream_);
+  graph_.capture(stream(), key, step);
+  graph_.launch(stream());
 }
 
 // =============================================================================================
@@ -603,8 +570,8 @@ void Translator::run_search(const BeamState& bs, int64_t S, int64_t first_check)
     launch_or_capture_step(bs, S, key);
     if (s + 1 == bs.max_steps) break;
     if (s >= first_check && (s - first_check) % poll == poll - 1) {
-      CT2_CUDA_CHECK(cudaMemcpyAsync(hfin, bs.num_finished, 4, cudaMemcpyDeviceToHost, stream_));
-      CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));
+      CT2_CUDA_CHECK(cudaMemcpyAsync(hfin, bs.num_finished, 4, cudaMemcpyDeviceToHost, stream()));
+      CT2_CUDA_CHECK(cudaStreamSynchronize(stream()));
       if (*hfin >= bs.batch) break;
     }
   }
@@ -642,10 +609,10 @@ std::vector<TranslationHypotheses> Translator::translate(const TranslationReques
   for (int64_t b = 0; b < B; ++b) hl[b] = r.source_lens[b];
   int32_t* hend = hl + B;
   for (size_t i = 0; i < r.end_ids.size(); ++i) hend[i] = r.end_ids[i];
-  CT2_CUDA_CHECK(cudaMemcpyAsync(src_ids_.ptr, hp, B * S * 4, cudaMemcpyHostToDevice, stream_));
-  CT2_CUDA_CHECK(cudaMemcpyAsync(src_lens_.ptr, hl, B * 4, cudaMemcpyHostToDevice, stream_));
+  CT2_CUDA_CHECK(cudaMemcpyAsync(src_ids_.ptr, hp, B * S * 4, cudaMemcpyHostToDevice, stream()));
+  CT2_CUDA_CHECK(cudaMemcpyAsync(src_lens_.ptr, hl, B * 4, cudaMemcpyHostToDevice, stream()));
   if (!r.end_ids.empty())
-    CT2_CUDA_CHECK(cudaMemcpyAsync(beam_.end_ids.ptr, hend, r.end_ids.size() * 4, cudaMemcpyHostToDevice, stream_));
+    CT2_CUDA_CHECK(cudaMemcpyAsync(beam_.end_ids.ptr, hend, r.end_ids.size() * 4, cudaMemcpyHostToDevice, stream()));
 
   // ---- encoder + memory projections ----
   run_encoder(B, S);
@@ -655,9 +622,9 @@ std::vector<TranslationHypotheses> Translator::translate(const TranslationReques
   BeamState bs = beam_.state(B, beam, mc_.tgt_vocab, L, r.min_decoding_length, r.patience, r.length_penalty, r.num_hypotheses,
                              static_cast<int>(r.end_ids.size()));
   set_logits_ld(bs);
-  beam_.reset(bs, r.start_id, dtype_, stream_);
+  beam_.reset(bs, r.start_id, dtype_, stream());
   run_search(bs, S, std::max<int64_t>(0, r.min_decoding_length));
-  return beam_.collect(bs, r.length_penalty, r.num_hypotheses, r.return_end_token ? std::vector<int32_t>{} : r.end_ids, stream_);
+  return beam_.collect(bs, r.length_penalty, r.num_hypotheses, r.return_end_token ? std::vector<int32_t>{} : r.end_ids, stream());
 }
 
 // =============================================================================================
@@ -675,7 +642,7 @@ bool Translator::decode_teacher_forced(int64_t entries, int64_t T, int64_t S, co
   const float scale = 1.f / std::sqrt(static_cast<float>(mc_.head_dim));
   embed_decoder(ids_d, entries * T, T, nullptr);
   return run_decoder_layers(entries * T, static_cast<int>(T), S, [&](int) {
-    launch_attention_causal(qkv_.ptr, entries, static_cast<int>(T), mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, dtype_, stream_);
+    launch_attention_causal(qkv_.ptr, entries, static_cast<int>(T), mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, dtype_, stream());
   }, capture);
 }
 
@@ -685,7 +652,7 @@ void Translator::project_rows(const int32_t* rows_d, int64_t n, bool xq,
   CT2_REQUIRE(rows_d || n <= score_slab_rows_, "project_rows: rows projected in place must fit one slab");
   for (int64_t c = 0; c < n; c += score_slab_rows_) {
     const int64_t k = std::min(score_slab_rows_, n - c);
-    if (rows_d) launch_gather_rows(x_.ptr, rows_d + c, k, mc_.d_model * dtype_size(dtype_), q_.ptr, stream_);
+    if (rows_d) launch_gather_rows(x_.ptr, rows_d + c, k, mc_.d_model * dtype_size(dtype_), q_.ptr, stream());
     dense(projection_, mc_.has_dec_final_norm ? &dec_norm_ : nullptr, rows_d ? q_.ptr : x_.ptr, k, nullptr, -1,
           score_logits_.ptr, !rows_d && xq, ld);
     reduce(score_logits_.ptr, c, k, ld);
@@ -695,7 +662,7 @@ void Translator::project_rows(const int32_t* rows_d, int64_t n, bool xq,
 const int32_t* Translator::stage_ids(const std::vector<int32_t>& ids) {
   const size_t bytes = ids.size() * sizeof(int32_t);
   if (score_ids_.bytes < bytes) score_ids_.alloc(bytes);
-  CT2_CUDA_CHECK(cudaMemcpyAsync(score_ids_.ptr, ids.data(), bytes, cudaMemcpyHostToDevice, stream_));
+  CT2_CUDA_CHECK(cudaMemcpyAsync(score_ids_.ptr, ids.data(), bytes, cudaMemcpyHostToDevice, stream()));
   return score_ids_.as<int32_t>();
 }
 
@@ -754,8 +721,8 @@ void Translator::score(const int32_t* src_ids_h, const int32_t* src_lens_h, int6
     ensure_rows(nb, nb * Sp, std::max(rows, nb * Sp));     // no search state: the beam arena and self K/V keep their size
     if (score_out_.bytes < np * sizeof(float)) score_out_.alloc(np * sizeof(float));
     float* scores_d = score_out_.as<float>();
-    CT2_CUDA_CHECK(cudaMemcpyAsync(src_ids_.ptr, src.data(), src.size() * 4, cudaMemcpyHostToDevice, stream_));
-    CT2_CUDA_CHECK(cudaMemcpyAsync(src_lens_.ptr, lens.data(), nb * 4, cudaMemcpyHostToDevice, stream_));
+    CT2_CUDA_CHECK(cudaMemcpyAsync(src_ids_.ptr, src.data(), src.size() * 4, cudaMemcpyHostToDevice, stream()));
+    CT2_CUDA_CHECK(cudaMemcpyAsync(src_lens_.ptr, lens.data(), nb * 4, cudaMemcpyHostToDevice, stream()));
     const int32_t* dec_d = stage_ids(staged);
     const int32_t* picked_d = dec_d + rows;
     const int32_t* targets_d = picked_d + np;
@@ -764,11 +731,11 @@ void Translator::score(const int32_t* src_ids_h, const int32_t* src_lens_h, int6
     project_memory(nb, Sp);
     decode_teacher_forced(nb, Tp, Sp, dec_d);
     project_rows(picked_d, np, false, [&](const void* logits, int64_t c, int64_t k, int64_t ld) {
-      launch_log_softmax_gather(logits, targets_d + c, k, V, scores_d + c, dtype_, stream_, ld);
+      launch_log_softmax_gather(logits, targets_d + c, k, V, scores_d + c, dtype_, stream(), ld);
     });
     std::vector<float> vals(np);
-    CT2_CUDA_CHECK(cudaMemcpyAsync(vals.data(), scores_d, np * sizeof(float), cudaMemcpyDeviceToHost, stream_));
-    CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));     // also keeps the staging vectors alive until their copies are done
+    CT2_CUDA_CHECK(cudaMemcpyAsync(vals.data(), scores_d, np * sizeof(float), cudaMemcpyDeviceToHost, stream()));
+    CT2_CUDA_CHECK(cudaStreamSynchronize(stream()));     // also keeps the staging vectors alive until their copies are done
     for (int64_t i = 0; i < np; ++i) out_h[dest[i]] = vals[i];
   }
 }
@@ -795,17 +762,17 @@ void Translator::encode(const int32_t* ids_h, const int32_t* lens_h, int64_t bat
     CT2_REQUIRE(lens_h[b] >= 1 && lens_h[b] <= S, "encode: source lengths must be in [1, max_source_len]");
     for (int64_t t = 0; t < S; ++t) hp[b * S + t] = t < lens_h[b] ? ids_h[b * S + t] : 0;
   }
-  CT2_CUDA_CHECK(cudaMemcpyAsync(src_ids_.ptr, hp, batch * S * 4, cudaMemcpyHostToDevice, stream_));
-  CT2_CUDA_CHECK(cudaMemcpyAsync(src_lens_.ptr, lens_h, batch * 4, cudaMemcpyHostToDevice, stream_));
+  CT2_CUDA_CHECK(cudaMemcpyAsync(src_ids_.ptr, hp, batch * S * 4, cudaMemcpyHostToDevice, stream()));
+  CT2_CUDA_CHECK(cudaMemcpyAsync(src_lens_.ptr, lens_h, batch * 4, cudaMemcpyHostToDevice, stream()));
   run_encoder(batch, S);
   copy_memory_to_host(batch * S, memory_h);
 }
 
 void Translator::copy_memory_to_host(int64_t rows, float* memory_h) {
   DeviceBuffer f32(static_cast<size_t>(rows) * mc_.d_model * 4);
-  launch_convert_to_f32(memory_.ptr, rows * mc_.d_model, f32.as<float>(), dtype_, stream_);
-  CT2_CUDA_CHECK(cudaMemcpyAsync(memory_h, f32.ptr, f32.bytes, cudaMemcpyDeviceToHost, stream_));
-  CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));
+  launch_convert_to_f32(memory_.ptr, rows * mc_.d_model, f32.as<float>(), dtype_, stream());
+  CT2_CUDA_CHECK(cudaMemcpyAsync(memory_h, f32.ptr, f32.bytes, cudaMemcpyDeviceToHost, stream()));
+  CT2_CUDA_CHECK(cudaStreamSynchronize(stream()));
 }
 
 void Translator::bench(int64_t batch, int64_t source_len, int beam, int64_t steps, int64_t warmup, float* encode_ms,
@@ -829,20 +796,20 @@ void Translator::bench(int64_t batch, int64_t source_len, int beam, int64_t step
   cudaEventCreate(&e3);
   run_encoder(batch, source_len);      // warm-up (first-use kernel configuration)
   project_memory(batch, source_len);
-  CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));
-  cudaEventRecord(e0, stream_);
+  CT2_CUDA_CHECK(cudaStreamSynchronize(stream()));
+  cudaEventRecord(e0, stream());
   run_encoder(batch, source_len);
   project_memory(batch, source_len);
-  cudaEventRecord(e1, stream_);
-  beam_.reset(bs, 1, dtype_, stream_);
+  cudaEventRecord(e1, stream());
+  beam_.reset(bs, 1, dtype_, stream());
   for (int64_t s = 0; s < warmup; ++s) launch_or_capture_step(bs, source_len, key);
-  CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));
+  CT2_CUDA_CHECK(cudaStreamSynchronize(stream()));
   const int64_t l0 = g_kernel_launches.load();
   cudaProfilerStart();
-  cudaEventRecord(e2, stream_);
+  cudaEventRecord(e2, stream());
   for (int64_t s = 0; s < steps; ++s) launch_or_capture_step(bs, source_len, key);
-  cudaEventRecord(e3, stream_);
-  CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));
+  cudaEventRecord(e3, stream());
+  CT2_CUDA_CHECK(cudaStreamSynchronize(stream()));
   cudaProfilerStop();
   *launches = g_kernel_launches.load() - l0;
   cudaEventElapsedTime(encode_ms, e0, e1);
@@ -861,16 +828,16 @@ void Translator::bench(int64_t batch, int64_t source_len, int beam, int64_t step
 void Translator::run_encoder_only(int64_t batch, int64_t S) {
   const int64_t rows = batch * S, d = mc_.d_model;
   launch_embed_pos(enc_emb_.weight.ptr, enc_emb_.kind == DenseWeights::INT8 ? enc_emb_.scale.as<float>() : nullptr,
-                   src_ids_.as<int32_t>(), rows, d, mc_.enc_emb_scale, enc_pos_.ptr, S, nullptr, false, x_.ptr, dtype_, stream_,
+                   src_ids_.as<int32_t>(), rows, d, mc_.enc_emb_scale, enc_pos_.ptr, S, nullptr, false, x_.ptr, dtype_, stream(),
                    mc_.type_vocab ? type_emb_.weight.ptr : nullptr,
                    type_emb_.kind == DenseWeights::INT8 ? type_emb_.scale.as<float>() : nullptr, type_ids_.as<int32_t>());
   if (mc_.has_emb_norm)
     launch_layer_norm(x_.ptr, emb_norm_.gamma.ptr, emb_norm_.beta.ptr, rows, d, mc_.eps, x_.ptr, nullptr, nullptr, true, dtype_,
-                      stream_);
+                      stream());
   run_encoder_layers(batch, S, src_lens_.as<int32_t>());
   if (mc_.has_pooler) {
     const size_t es = dtype_size(dtype_);
-    CT2_CUDA_CHECK(cudaMemcpy2DAsync(first_.ptr, d * es, memory_.ptr, S * d * es, d * es, batch, cudaMemcpyDeviceToDevice, stream_));
+    CT2_CUDA_CHECK(cudaMemcpy2DAsync(first_.ptr, d * es, memory_.ptr, S * d * es, d * es, batch, cudaMemcpyDeviceToDevice, stream()));
     dense(pooler_, nullptr, first_.ptr, batch, nullptr, mc_.pooler_activation, pooled_.ptr);
   }
 }
@@ -908,15 +875,15 @@ void Translator::encoder_forward(const int32_t* ids_h, const int32_t* types_h, c
     first_.alloc(batch * mc_.d_model * es);
     pooled_.alloc(batch * mc_.d_model * es);
   }
-  CT2_CUDA_CHECK(cudaMemcpyAsync(src_ids_.ptr, ids.data(), ids.size() * 4, cudaMemcpyHostToDevice, stream_));
-  CT2_CUDA_CHECK(cudaMemcpyAsync(type_ids_.ptr, types.data(), types.size() * 4, cudaMemcpyHostToDevice, stream_));
-  CT2_CUDA_CHECK(cudaMemcpyAsync(src_lens_.ptr, lens_h, batch * 4, cudaMemcpyHostToDevice, stream_));
+  CT2_CUDA_CHECK(cudaMemcpyAsync(src_ids_.ptr, ids.data(), ids.size() * 4, cudaMemcpyHostToDevice, stream()));
+  CT2_CUDA_CHECK(cudaMemcpyAsync(type_ids_.ptr, types.data(), types.size() * 4, cudaMemcpyHostToDevice, stream()));
+  CT2_CUDA_CHECK(cudaMemcpyAsync(src_lens_.ptr, lens_h, batch * 4, cudaMemcpyHostToDevice, stream()));
   run_encoder_only(batch, T);
   if (mc_.has_pooler && pooled_h) {
     DeviceBuffer f32(static_cast<size_t>(batch) * mc_.d_model * 4);
-    launch_convert_to_f32(pooled_.ptr, batch * mc_.d_model, f32.as<float>(), dtype_, stream_);
-    CT2_CUDA_CHECK(cudaMemcpyAsync(pooled_h, f32.ptr, f32.bytes, cudaMemcpyDeviceToHost, stream_));
-    CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    launch_convert_to_f32(pooled_.ptr, batch * mc_.d_model, f32.as<float>(), dtype_, stream());
+    CT2_CUDA_CHECK(cudaMemcpyAsync(pooled_h, f32.ptr, f32.bytes, cudaMemcpyDeviceToHost, stream()));
+    CT2_CUDA_CHECK(cudaStreamSynchronize(stream()));
   }
   copy_memory_to_host(batch * T, hidden_h);     // synchronises: ids / types may go
 }
@@ -933,10 +900,10 @@ void Translator::encoder_bench(const int32_t* lens_h, int64_t batch, int64_t T, 
   cudaEventCreate(&e1);
   std::vector<float> ms;
   for (int64_t i = 0; i < warmup + iters; ++i) {
-    cudaEventRecord(e0, stream_);
+    cudaEventRecord(e0, stream());
     run_encoder_only(batch, T);
-    cudaEventRecord(e1, stream_);
-    CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    cudaEventRecord(e1, stream());
+    CT2_CUDA_CHECK(cudaStreamSynchronize(stream()));
     float t = 0.f;
     cudaEventElapsedTime(&t, e0, e1);
     if (i >= warmup) ms.push_back(t);
@@ -961,14 +928,14 @@ int64_t Translator::whisper_positions(int64_t batch, int64_t frames) const {
 void Translator::encode_audio(const float* features_h, int64_t batch, int64_t frames) {
   const int64_t d = mc_.d_model, S = whisper_positions(batch, frames);
   audio_lens_h_.assign(batch, static_cast<int32_t>(S));
-  CT2_CUDA_CHECK(cudaMemcpyAsync(features_.ptr, features_h, batch * mc_.n_mels * frames * 4, cudaMemcpyHostToDevice, stream_));
-  CT2_CUDA_CHECK(cudaMemcpyAsync(src_lens_.ptr, audio_lens_h_.data(), batch * 4, cudaMemcpyHostToDevice, stream_));
-  launch_im2col(features_.ptr, true, batch, mc_.n_mels, frames, frames, 3, 1, 1, true, cols_.ptr, dtype_, stream_);
+  CT2_CUDA_CHECK(cudaMemcpyAsync(features_.ptr, features_h, batch * mc_.n_mels * frames * 4, cudaMemcpyHostToDevice, stream()));
+  CT2_CUDA_CHECK(cudaMemcpyAsync(src_lens_.ptr, audio_lens_h_.data(), batch * 4, cudaMemcpyHostToDevice, stream()));
+  launch_im2col(features_.ptr, true, batch, mc_.n_mels, frames, frames, 3, 1, 1, true, cols_.ptr, dtype_, stream());
   gemm_float(cols_.ptr, conv1_.weight.ptr, conv1_.bias.ptr, nullptr, CT2B200_ACT_GELU, batch * frames, d, mc_.n_mels * 3,
-             conv_out_.ptr, dtype_, stream_);
-  launch_im2col(conv_out_.ptr, false, batch, d, frames, S, 3, 2, 1, false, cols_.ptr, dtype_, stream_);
-  gemm_float(cols_.ptr, conv2_.weight.ptr, conv2_.bias.ptr, nullptr, CT2B200_ACT_GELU, batch * S, d, d * 3, x_.ptr, dtype_, stream_);
-  launch_add_positions(x_.ptr, enc_pos_.ptr, batch * S, S, d, dtype_, stream_);
+             conv_out_.ptr, dtype_, stream());
+  launch_im2col(conv_out_.ptr, false, batch, d, frames, S, 3, 2, 1, false, cols_.ptr, dtype_, stream());
+  gemm_float(cols_.ptr, conv2_.weight.ptr, conv2_.bias.ptr, nullptr, CT2B200_ACT_GELU, batch * S, d, d * 3, x_.ptr, dtype_, stream());
+  launch_add_positions(x_.ptr, enc_pos_.ptr, batch * S, S, d, dtype_, stream());
   run_encoder_layers(batch, S, nullptr);
 }
 
@@ -1034,10 +1001,10 @@ std::vector<TranslationHypotheses> Translator::whisper_generate(const WhisperReq
   const size_t nsup = r.suppress_ids.size() + r.suppress_ids_begin.size();
   forced_d_.alloc(P * N * 4);
   suppress_d_.alloc((nsup + 1) * 4);
-  CT2_CUDA_CHECK(cudaMemcpyAsync(forced_d_.ptr, hp, P * N * 4, cudaMemcpyHostToDevice, stream_));
-  CT2_CUDA_CHECK(cudaMemcpyAsync(suppress_d_.ptr, hs, (nsup + 1) * 4, cudaMemcpyHostToDevice, stream_));
-  CT2_CUDA_CHECK(cudaMemcpyAsync(beam_.end_ids.ptr, suppress_d_.as<int32_t>() + nsup, 4, cudaMemcpyDeviceToDevice, stream_));
-  CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));      // the pinned staging is reused below
+  CT2_CUDA_CHECK(cudaMemcpyAsync(forced_d_.ptr, hp, P * N * 4, cudaMemcpyHostToDevice, stream()));
+  CT2_CUDA_CHECK(cudaMemcpyAsync(suppress_d_.ptr, hs, (nsup + 1) * 4, cudaMemcpyHostToDevice, stream()));
+  CT2_CUDA_CHECK(cudaMemcpyAsync(beam_.end_ids.ptr, suppress_d_.as<int32_t>() + nsup, 4, cudaMemcpyDeviceToDevice, stream()));
+  CT2_CUDA_CHECK(cudaStreamSynchronize(stream()));      // the pinned staging is reused below
 
   // ---- encoder + memory projections ----
   encode_audio(r.features, B, frames);
@@ -1059,18 +1026,18 @@ std::vector<TranslationHypotheses> Translator::whisper_generate(const WhisperReq
     bs.ts_no_timestamps = r.no_timestamps_id;
     bs.ts_max_initial = bs.ts_begin + r.max_initial_timestamp_index;
   }
-  beam_.reset(bs, r.prompts[0], dtype_, stream_);
-  if (sampling) beam_.reset_sampling(bs, r.sampling_topk, r.sampling_temperature, stream_);
-  CT2_CUDA_CHECK(cudaMemcpyAsync(beam_.next_ids.ptr, forced_d_.ptr, N * 4, cudaMemcpyDeviceToDevice, stream_));
+  beam_.reset(bs, r.prompts[0], dtype_, stream());
+  if (sampling) beam_.reset_sampling(bs, r.sampling_topk, r.sampling_temperature, stream());
+  CT2_CUDA_CHECK(cudaMemcpyAsync(beam_.next_ids.ptr, forced_d_.ptr, N * 4, cudaMemcpyDeviceToDevice, stream()));
   no_speech_d_.alloc(B * 4);
   for (int64_t t = 0; t < start_step; ++t) {
     decoder_step(N, beam, B, S);
     if (no_speech_h && t == sot_index) {
       CT2_REQUIRE(r.no_speech_id >= 0, "return_no_speech_prob needs the id of <|nospeech|>");
       launch_token_prob(logits_.ptr, B, mc_.tgt_vocab, static_cast<int64_t>(beam) * logits_ld_, r.no_speech_id,
-                        no_speech_d_.as<float>(), dtype_, stream_);
+                        no_speech_d_.as<float>(), dtype_, stream());
     }
-    launch_beam_force(bs, forced_d_.as<int32_t>() + (t + 1) * N, stream_);
+    launch_beam_force(bs, forced_d_.as<int32_t>() + (t + 1) * N, stream());
   }
   CT2_REQUIRE(!no_speech_h || sot_index < start_step, "return_no_speech_prob with <|startoftranscript|> as the last prompt "
                                                       "token is not supported");
@@ -1078,10 +1045,10 @@ std::vector<TranslationHypotheses> Translator::whisper_generate(const WhisperReq
   // ---- search ----
   run_search(bs, S, 0);
   if (no_speech_h) {
-    CT2_CUDA_CHECK(cudaMemcpyAsync(no_speech_h, no_speech_d_.ptr, B * 4, cudaMemcpyDeviceToHost, stream_));
-    CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    CT2_CUDA_CHECK(cudaMemcpyAsync(no_speech_h, no_speech_d_.ptr, B * 4, cudaMemcpyDeviceToHost, stream()));
+    CT2_CUDA_CHECK(cudaStreamSynchronize(stream()));
   }
-  return beam_.collect(bs, r.length_penalty, r.num_hypotheses, {}, stream_);
+  return beam_.collect(bs, r.length_penalty, r.num_hypotheses, {}, stream());
 }
 
 // =============================================================================================
@@ -1125,7 +1092,7 @@ std::vector<WhisperAlignResult> Translator::whisper_align(const WhisperAlignRequ
     masks[static_cast<size_t>(layer) * H + head] |= 1u << count[layer]++;
   }
   if (align_masks_.bytes < masks.size() * 4) align_masks_.alloc(masks.size() * 4);
-  CT2_CUDA_CHECK(cudaMemcpyAsync(align_masks_.ptr, masks.data(), masks.size() * 4, cudaMemcpyHostToDevice, stream_));
+  CT2_CUDA_CHECK(cudaMemcpyAsync(align_masks_.ptr, masks.data(), masks.size() * 4, cudaMemcpyHostToDevice, stream()));
   std::vector<AttnCapture> capture(mc_.dec_layers);
   for (int l = 0, first = 0; l < mc_.dec_layers; ++l) {
     capture[l].masks = count[l] ? align_masks_.as<uint32_t>() + static_cast<size_t>(l) * H : nullptr;
@@ -1201,21 +1168,21 @@ std::vector<WhisperAlignResult> Translator::whisper_align(const WhisperAlignRequ
     for (auto& c : capture) c.out = align_scores_.as<float>();
     decode_teacher_forced(nb, Tp, S, dec_d, &capture);
     project_rows(picked_d, np, false, [&](const void* logits, int64_t c, int64_t k, int64_t ld) {
-      launch_softmax_gather(logits, targets_d + c, k, r.eot_id, ld, probs_d + c, dtype_, stream_);
+      launch_softmax_gather(logits, targets_d + c, k, r.eot_id, ld, probs_d + c, dtype_, stream());
     });
     std::vector<float> probs(np), matrix;
     if (!all_zero) {
       float* sc = align_scores_.as<float>();
-      launch_align_softmax(sc, nf_d, len_d, nb, Hs, Tp, S, dtype_, stream_);
+      launch_align_softmax(sc, nf_d, len_d, nb, Hs, Tp, S, dtype_, stream());
       launch_align_standardize(sc, nf_d, len_d, ntext_d, nb, Hs, Tp, S, equal ? Tg : 0, s0, Nt, S, align_norm_.as<float>(), dtype_,
-                               stream_);
+                               stream());
       launch_align_median_mean(align_norm_.as<float>(), nf_d, ntext_d, nb, Hs, Nt, S, width, align_matrix_.as<float>(), dtype_,
-                               stream_);
+                               stream());
       matrix.resize(nb * (Nt + 1) * S);
-      CT2_CUDA_CHECK(cudaMemcpyAsync(matrix.data(), align_matrix_.ptr, matrix_bytes, cudaMemcpyDeviceToHost, stream_));
+      CT2_CUDA_CHECK(cudaMemcpyAsync(matrix.data(), align_matrix_.ptr, matrix_bytes, cudaMemcpyDeviceToHost, stream()));
     }
-    if (np) CT2_CUDA_CHECK(cudaMemcpyAsync(probs.data(), probs_d, np * sizeof(float), cudaMemcpyDeviceToHost, stream_));
-    CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));     // also keeps the staging vectors alive until their copies are done
+    if (np) CT2_CUDA_CHECK(cudaMemcpyAsync(probs.data(), probs_d, np * sizeof(float), cudaMemcpyDeviceToHost, stream()));
+    CT2_CUDA_CHECK(cudaStreamSynchronize(stream()));     // also keeps the staging vectors alive until their copies are done
     int64_t k = 0;
     for (int64_t b = 0; b < nb; ++b) {
       const int64_t g = p0 + b, n = r.text_lens[g];
@@ -1259,10 +1226,10 @@ void Translator::whisper_detect_language(const float* features_h, int64_t batch,
     project_memory(nb, S);
     const bool xq = decode_teacher_forced(nb, 1, S, ids_d);
     project_rows(nullptr, nb, xq, [&](const void* logits, int64_t c, int64_t k, int64_t ld) {
-      launch_gather_softmax(logits, k, ld, ids_d + nb, n, probs_d + c * n, dtype_, stream_);
+      launch_gather_softmax(logits, k, ld, ids_d + nb, n, probs_d + c * n, dtype_, stream());
     });
-    CT2_CUDA_CHECK(cudaMemcpyAsync(probs_h + p0 * n, score_out_.ptr, nb * n * sizeof(float), cudaMemcpyDeviceToHost, stream_));
-    CT2_CUDA_CHECK(cudaStreamSynchronize(stream_));
+    CT2_CUDA_CHECK(cudaMemcpyAsync(probs_h + p0 * n, score_out_.ptr, nb * n * sizeof(float), cudaMemcpyDeviceToHost, stream()));
+    CT2_CUDA_CHECK(cudaStreamSynchronize(stream()));
   }
 }
 

@@ -163,7 +163,7 @@ class Translator {
              int64_t* launches);
 
  private:
-  void load_dense(const ModelFile& f, const std::string& prefix, DenseWeights& w);
+  cudaStream_t stream() const { return gpu_.stream; }
   void load_norm(const ModelFile& f, const std::string& prefix, NormWeights& n);
   void drop_graph();            // synchronises and destroys the captured step (its buffers are about to move)
   void ensure_arena(int64_t batch, int64_t src_len, int beam, int64_t max_steps);
@@ -215,9 +215,8 @@ class Translator {
 
   std::mutex mu_;                // translate / score / encode / bench are serialised per translator
   Seq2SeqConfig mc_;
-  int dtype_ = CT2B200_F32, device_ = 0, weight_type_ = CT2B200_WEIGHTS_STORED, sm_count_ = 132;
+  int dtype_ = CT2B200_F32;
   bool use_graph_ = true;
-  cudaStream_t stream_ = nullptr;
 
   DenseWeights enc_emb_, dec_emb_, projection_;
   DenseWeights type_emb_, pooler_;   // encoder-only models: token-type embeddings, pooler_dense
@@ -253,6 +252,8 @@ class Translator {
   DeviceBuffer align_scores_, align_norm_, align_matrix_, align_masks_;
 
   StepGraph graph_;
+  // last: it is destroyed first, so the stream is synchronised before any buffer above is freed
+  EngineDevice gpu_;
 };
 
 }  // namespace ct2b200
