@@ -663,6 +663,30 @@ CT2B200_API int ct2b200_translator_summary(const char* model_dir, char* json_out
   });
 }
 
+namespace {
+// the TranslationRequest of ct2b200_translate_batch's arguments (the logits processors left off)
+TranslationRequest translation_request(const int32_t* source_ids, const int32_t* source_lens, int64_t batch, int64_t max_source_len,
+                                       int beam_size, float patience, float length_penalty, int64_t max_decoding_length,
+                                       int64_t min_decoding_length, int num_hypotheses, int32_t start_id, const int32_t* end_ids,
+                                       int num_end_ids, int return_end_token) {
+  TranslationRequest r;
+  r.source_ids = source_ids;
+  r.source_lens = source_lens;
+  r.batch = batch;
+  r.max_source_len = max_source_len;
+  r.beam_size = beam_size;
+  r.patience = patience;
+  r.length_penalty = length_penalty;
+  r.max_decoding_length = max_decoding_length;
+  r.min_decoding_length = min_decoding_length;
+  r.num_hypotheses = num_hypotheses;
+  r.start_id = start_id;
+  r.end_ids.assign(end_ids, end_ids + (end_ids ? num_end_ids : 0));
+  r.return_end_token = return_end_token != 0;
+  return r;
+}
+}  // namespace
+
 CT2B200_API int ct2b200_translate_batch(ct2b200_translator* t, const int32_t* source_ids, const int32_t* source_lens, int64_t batch,
                             int64_t max_source_len, int beam_size, float patience, float length_penalty,
                             int64_t max_decoding_length, int64_t min_decoding_length, int num_hypotheses, int32_t start_id,
@@ -670,20 +694,39 @@ CT2B200_API int ct2b200_translate_batch(ct2b200_translator* t, const int32_t* so
                             float* out_scores) {
   return guarded([&] {
     CT2_REQUIRE(t && source_ids && source_lens && out_ids && out_lens && out_scores, "translate_batch: null argument");
-    TranslationRequest r;
-    r.source_ids = source_ids;
-    r.source_lens = source_lens;
-    r.batch = batch;
-    r.max_source_len = max_source_len;
-    r.beam_size = beam_size;
-    r.patience = patience;
-    r.length_penalty = length_penalty;
-    r.max_decoding_length = max_decoding_length;
-    r.min_decoding_length = min_decoding_length;
-    r.num_hypotheses = num_hypotheses;
-    r.start_id = start_id;
-    r.end_ids.assign(end_ids, end_ids + (end_ids ? num_end_ids : 0));
-    r.return_end_token = return_end_token != 0;
+    const TranslationRequest r = translation_request(source_ids, source_lens, batch, max_source_len, beam_size, patience,
+                                                     length_penalty, max_decoding_length, min_decoding_length, num_hypotheses,
+                                                     start_id, end_ids, num_end_ids, return_end_token);
+    copy_hypotheses(t->impl->translate(r), batch, num_hypotheses, max_decoding_length, out_ids, out_lens, out_scores);
+  });
+}
+
+CT2B200_API int ct2b200_translate_batch_processors(ct2b200_translator* t, const int32_t* source_ids, const int32_t* source_lens,
+                            int64_t batch, int64_t max_source_len, int beam_size, float patience, float length_penalty,
+                            int64_t max_decoding_length, int64_t min_decoding_length, int num_hypotheses, int32_t start_id,
+                            const int32_t* end_ids, int num_end_ids, int return_end_token, float repetition_penalty,
+                            int no_repeat_ngram_size, const int32_t* disable_ids, int num_disable_ids,
+                            const int32_t* sequence_ids, const int32_t* sequence_offsets, int num_sequences, int32_t* out_ids,
+                            int32_t* out_lens, float* out_scores) {
+  return guarded([&] {
+    CT2_REQUIRE(t && source_ids && source_lens && out_ids && out_lens && out_scores, "translate_batch: null argument");
+    CT2_REQUIRE(num_disable_ids >= 0 && num_sequences >= 0, "translate_batch: negative count");
+    CT2_REQUIRE((num_disable_ids == 0 || disable_ids) && (num_sequences == 0 || sequence_offsets),
+                "translate_batch: null processor table");
+    CT2_REQUIRE(num_sequences <= kMaxSuppressSequences, "suppress_sequences: at most 4096 sequences");
+    TranslationRequest r = translation_request(source_ids, source_lens, batch, max_source_len, beam_size, patience, length_penalty,
+                                               max_decoding_length, min_decoding_length, num_hypotheses, start_id, end_ids,
+                                               num_end_ids, return_end_token);
+    r.repetition_penalty = repetition_penalty;
+    r.no_repeat_ngram_size = no_repeat_ngram_size;
+    r.disable_ids.assign(disable_ids, disable_ids + num_disable_ids);
+    if (num_sequences > 0) {
+      r.sequence_offsets.assign(sequence_offsets, sequence_offsets + num_sequences + 1);
+      const int32_t total = r.sequence_offsets.back();
+      CT2_REQUIRE(total >= 0 && total <= kMaxSuppressSequenceTokens && (total == 0 || sequence_ids),
+                  "suppress_sequences: at most 65536 tokens in all");
+      r.sequence_ids.assign(sequence_ids, sequence_ids + total);
+    }
     copy_hypotheses(t->impl->translate(r), batch, num_hypotheses, max_decoding_length, out_ids, out_lens, out_scores);
   });
 }

@@ -88,6 +88,34 @@ BeamState BeamSearchArena::state(int64_t batch, int beam, int64_t vocab, int64_t
   return bs;
 }
 
+bool BeamSearchArena::ensure_processors(size_t elems) {
+  if (elems * 4 <= processors.bytes) return false;
+  processors.alloc(std::max<size_t>(elems, 256) * 4);
+  return true;
+}
+
+void BeamSearchArena::set_processors(BeamState& bs, float repetition_penalty, int no_repeat_ngram_size,
+                                     const std::vector<int32_t>& disable_ids, const std::vector<int32_t>& sequence_offsets,
+                                     const std::vector<int32_t>& sequence_ids, cudaStream_t st) {
+  bs.rep_penalty = repetition_penalty != 1.f ? repetition_penalty : 0.f;
+  bs.no_repeat_ngram = no_repeat_ngram_size;
+  std::vector<int32_t> table(disable_ids);
+  table.insert(table.end(), sequence_offsets.begin(), sequence_offsets.end());
+  table.insert(table.end(), sequence_ids.begin(), sequence_ids.end());
+  if (table.empty()) return;
+  CT2_REQUIRE(table.size() * 4 <= processors.bytes, "set_processors: the table buffer was not grown");
+  // pageable source: the call returns once the table is staged, so the vector may go
+  CT2_CUDA_CHECK(cudaMemcpyAsync(processors.ptr, table.data(), table.size() * 4, cudaMemcpyHostToDevice, st));
+  const int32_t* d = processors.as<int32_t>();
+  bs.num_disable = static_cast<int>(disable_ids.size());
+  bs.disable_ids = d;
+  if (!sequence_offsets.empty()) {
+    bs.num_sequences = static_cast<int>(sequence_offsets.size()) - 1;
+    bs.seq_offsets = d + disable_ids.size();
+    bs.seq_ids = bs.seq_offsets + sequence_offsets.size();
+  }
+}
+
 void BeamSearchArena::reset(const BeamState& bs, int32_t start_id, int dtype, cudaStream_t st) {
   CT2_CUDA_CHECK(cudaMemsetAsync(counters.ptr, 0, 64, st));
   CT2_CUDA_CHECK(cudaMemsetAsync(finished.ptr, 0, bs.batch * 4, st));

@@ -21,6 +21,7 @@ struct BeamSearchArena {
   DeviceBuffer cum, cand_scores, cand_ids, next_ids, end_ids, counters, finished, top_done, num_hyp, alive, anc, parent;
   DeviceBuffer hyp_tokens, hyp_len, hyp_score;
   DeviceBuffer rng, sample_ids, sample_logp, row_score, row_done;   // sampled search
+  DeviceBuffer processors;                // logits processors: [disabled ids | sequence offsets | sequence ids] int32
   int32_t* host = nullptr;                // pinned staging of the results
   size_t host_elems = 0;
 
@@ -34,6 +35,14 @@ struct BeamSearchArena {
   bool ensure(int64_t batch, int beam, int64_t steps, size_t elem_size);
   BeamState state(int64_t batch, int beam, int64_t vocab, int64_t max_steps, int64_t min_length, float patience,
                   float length_penalty, int num_hypotheses, int num_end) const;
+  // grows `processors` to `elems` ids; true when it was reallocated (captured graphs over it are stale then)
+  bool ensure_processors(size_t elems);
+  // the history-dependent logits processors of a search (decoding_utils.cc:40-150): penalty 1 and n-gram size 0 are off;
+  // disable_ids are disabled at every step (SuppressTokens); sequence s is sequence_ids[sequence_offsets[s] ..
+  // sequence_offsets[s + 1]) (SuppressSequences; no offsets = none).  Uploads the tables on st into `processors`, which
+  // ensure_processors has sized, and points bs at them.
+  void set_processors(BeamState& bs, float repetition_penalty, int no_repeat_ngram_size, const std::vector<int32_t>& disable_ids,
+                      const std::vector<int32_t>& sequence_offsets, const std::vector<int32_t>& sequence_ids, cudaStream_t st);
   // clears the counters / flags and starts every beam from start_id (beam 0 live, the others at the lowest score)
   void reset(const BeamState& bs, int32_t start_id, int dtype, cudaStream_t st);
   // one search step over logits [batch * beam, vocab] T (modified in place): log-probabilities + cumulative scores,

@@ -558,12 +558,13 @@ void Translator::launch_or_capture_step(const BeamState& bs, int64_t S, const st
 // the decoding loop: one captured step per position; the host only polls the "finished entries" counter
 void Translator::run_search(const BeamState& bs, int64_t S, int64_t first_check) {
   // everything the captured step bakes in (kernel arguments are values)
-  uint32_t temperature_bits;
+  uint32_t temperature_bits, penalty_bits;
   std::memcpy(&temperature_bits, &bs.sample_temperature, 4);
+  std::memcpy(&penalty_bits, &bs.rep_penalty, 4);
   std::vector<int64_t> key = {bs.batch, bs.beam, S, bs.vocab_ld, bs.stride, bs.max_steps, bs.min_length, bs.max_hyp, bs.max_candidates,
                               bs.num_hypotheses, bs.early_exit, bs.num_end, bs.start_step, bs.include_eos, bs.num_disable,
                               bs.num_begin, bs.ts_begin, bs.ts_end, bs.ts_eot, bs.ts_no_timestamps, bs.ts_max_initial,
-                              bs.sample_topk, temperature_bits};
+                              bs.sample_topk, temperature_bits, penalty_bits, bs.no_repeat_ngram, bs.num_sequences};
   const int64_t poll = eos_poll_interval();
   int32_t* hfin = beam_.host;
   for (int64_t s = 0; s < bs.max_steps; ++s) {
@@ -599,7 +600,24 @@ std::vector<TranslationHypotheses> Translator::translate(const TranslationReques
       CT2_REQUIRE(id >= 0 && id < mc_.src_vocab, "translate_batch: source id out of range");
     }
   }
+  CT2_REQUIRE(std::isfinite(r.repetition_penalty) && r.repetition_penalty > 0.f, "repetition_penalty must be positive and finite");
+  CT2_REQUIRE(r.no_repeat_ngram_size >= 0, "no_repeat_ngram_size must be >= 0");
+  const int64_t nseq = r.sequence_offsets.empty() ? 0 : static_cast<int64_t>(r.sequence_offsets.size()) - 1;
+  CT2_REQUIRE(static_cast<int64_t>(r.disable_ids.size()) <= kMaxSuppressSequences && nseq <= kMaxSuppressSequences &&
+                  static_cast<int64_t>(r.sequence_ids.size()) <= kMaxSuppressSequenceTokens,
+              "suppress_sequences: at most 4096 ids, 4096 sequences and 65536 tokens in all");
+  CT2_REQUIRE(r.sequence_offsets.empty() ? r.sequence_ids.empty()
+                                         : r.sequence_offsets.front() == 0 &&
+                                               r.sequence_offsets.back() == static_cast<int64_t>(r.sequence_ids.size()),
+              "suppress_sequences: offsets must start at 0 and end at the number of ids");
+  for (int64_t s = 0; s < nseq; ++s)
+    CT2_REQUIRE(r.sequence_offsets[s] <= r.sequence_offsets[s + 1], "suppress_sequences: offsets must not decrease");
+  for (const std::vector<int32_t>* ids : {&r.disable_ids, &r.sequence_ids})
+    for (int32_t id : *ids) CT2_REQUIRE(id >= 0 && id < mc_.tgt_vocab, "suppressed token id outside the target vocabulary");
   ensure_arena(B, S, beam, L);
+  const size_t table = r.disable_ids.size() + r.sequence_offsets.size() + r.sequence_ids.size();
+  if (table * 4 > beam_.processors.bytes) drop_graph();          // the captured step reads the tables through their address
+  beam_.ensure_processors(table);
 
   // ---- inputs ----
   int32_t* hp = host_pinned_;
@@ -622,6 +640,8 @@ std::vector<TranslationHypotheses> Translator::translate(const TranslationReques
   BeamState bs = beam_.state(B, beam, mc_.tgt_vocab, L, r.min_decoding_length, r.patience, r.length_penalty, r.num_hypotheses,
                              static_cast<int>(r.end_ids.size()));
   set_logits_ld(bs);
+  beam_.set_processors(bs, r.repetition_penalty, r.no_repeat_ngram_size, r.disable_ids, r.sequence_offsets, r.sequence_ids,
+                       stream());
   beam_.reset(bs, r.start_id, dtype_, stream());
   run_search(bs, S, std::max<int64_t>(0, r.min_decoding_length));
   return beam_.collect(bs, r.length_penalty, r.num_hypotheses, r.return_end_token ? std::vector<int32_t>{} : r.end_ids, stream());

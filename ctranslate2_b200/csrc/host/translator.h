@@ -74,7 +74,17 @@ struct TranslationRequest {
   int32_t start_id = 1;                   // decoder start token (<s>)
   std::vector<int32_t> end_ids;           // normally {</s>}
   bool return_end_token = false;
+  // the logits processors (make_logits_processors, decoding.cc:1099-1112), applied on the device in every search step; the
+  // defaults leave them off
+  float repetition_penalty = 1.f;         // > 0 and finite
+  int no_repeat_ngram_size = 0;
+  std::vector<int32_t> disable_ids;       // SuppressTokens (disable_unk: the target vocabulary's unknown-token id)
+  std::vector<int32_t> sequence_offsets;  // SuppressSequences: sequence s = sequence_ids[offsets[s] .. offsets[s + 1]);
+  std::vector<int32_t> sequence_ids;      //   no offsets = no sequences
 };
+// The reference takes any number of suppressed sequences; this engine refuses more than these, never truncates.
+constexpr int64_t kMaxSuppressSequences = 4096;      // sequences, and disabled ids
+constexpr int64_t kMaxSuppressSequenceTokens = 65536;  // tokens of all sequences together
 
 // models::Whisper::generate (include/ctranslate2/models/whisper.h:11-60, src/models/whisper.cc:232-390), prompts made of
 // previous-text tokens, <|startoftranscript|> and the task tokens (no text after them); the timestamp rules

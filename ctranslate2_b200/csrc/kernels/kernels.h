@@ -209,6 +209,12 @@ struct BeamState {
   int num_disable = 0, num_begin = 0;
   const int32_t* disable_ids = nullptr;     // SuppressTokens: disabled at every step
   const int32_t* disable_begin = nullptr;   // SuppressTokensBegin: disabled at the first search step
+  // The history-dependent logits processors (src/decoding_utils.cc:40-150), on each row's token history; zero = off.
+  float rep_penalty = 0.f;          // RepetitionPenalty: x < 0 ? x * p : x / p on every token of the history, once each
+  int no_repeat_ngram = 0;          // NoRepeatNgram: n-gram size
+  int num_sequences = 0;            // SuppressSequences: sequence s = seq_ids[seq_offsets[s] .. seq_offsets[s + 1]) (non-empty)
+  const int32_t* seq_ids = nullptr;
+  const int32_t* seq_offsets = nullptr;   // [num_sequences + 1]
   // Whisper's ApplyTimestampRules (src/models/whisper.cc:742-860); ts_begin = 0 disables them
   int ts_begin = 0, ts_end = 0, ts_eot = 0, ts_no_timestamps = 0, ts_max_initial = 0;
   const int32_t* end_ids = nullptr;

@@ -37,8 +37,7 @@ def translator_summary(model_path: str) -> dict:
 
 # TranslationOptions (include/ctranslate2/translation.h:14-98) this engine does not implement, with the only value it accepts
 _NEUTRAL = {
-    "coverage_penalty": 0, "repetition_penalty": 1, "no_repeat_ngram_size": 0, "disable_unk": False,
-    "suppress_sequences": None, "prefix_bias_beta": 0, "sampling_topk": 1, "sampling_topp": 1, "sampling_temperature": 1,
+    "coverage_penalty": 0, "prefix_bias_beta": 0, "sampling_topk": 1, "sampling_topp": 1, "sampling_temperature": 1,
     "use_vmap": False, "return_attention": False, "return_logits_vocab": False, "return_alternatives": False,
     "min_alternative_expansion_prob": 0, "replace_unknowns": False, "callback": None, "asynchronous": False,
     "max_batch_size": 0, "batch_type": "examples", "max_input_length": 1024,
@@ -55,6 +54,44 @@ def _neutral(name, value) -> bool:
         return value == neutral
     return not isinstance(value, (bool, np.bool_)) and isinstance(value, (int, float, np.integer, np.floating)) \
         and float(value) == float(neutral)
+
+
+# The engine's limits on the SuppressTokens / SuppressSequences tables (kMaxSuppressSequences, csrc/host/translator.h): larger
+# tables are refused, never truncated
+MAX_SUPPRESS_SEQUENCES = 4096
+MAX_SUPPRESS_SEQUENCE_TOKENS = 65536
+
+
+def _processor_options(repetition_penalty, no_repeat_ngram_size, disable_ids, suppress_sequences, vocab_size: int):
+    """Checks the logits processors in id form (types as the reference's Python bindings take them) and returns
+    (penalty, n, disabled ids, sequence offsets, sequence ids) for ct2b200_translate_batch_processors."""
+    if isinstance(repetition_penalty, (bool, np.bool_)) or not isinstance(repetition_penalty, (int, float, np.integer, np.floating)):
+        raise ValueError(f"repetition_penalty must be a number, not {type(repetition_penalty).__name__}")
+    penalty = float(repetition_penalty)
+    if not (np.isfinite(penalty) and penalty > 0):
+        raise ValueError(f"repetition_penalty must be positive and finite, got {repetition_penalty!r}")
+    if isinstance(no_repeat_ngram_size, (bool, np.bool_)) or not isinstance(no_repeat_ngram_size, (int, np.integer)) \
+            or no_repeat_ngram_size < 0:
+        raise ValueError(f"no_repeat_ngram_size must be a non-negative int, got {no_repeat_ngram_size!r}")
+    ids = [_token_id(i, "disabled id", vocab_size) for i in disable_ids]
+    offsets, flat = [0], []
+    for seq in suppress_sequences:
+        if isinstance(seq, (str, bytes)) or not hasattr(seq, "__len__"):
+            raise ValueError(f"suppress_sequences must hold token sequences, not {type(seq).__name__}")
+        flat += [_token_id(i, "suppressed sequence id", vocab_size) for i in seq]
+        offsets.append(len(flat))
+    if len(ids) > MAX_SUPPRESS_SEQUENCES or len(offsets) - 1 > MAX_SUPPRESS_SEQUENCES or len(flat) > MAX_SUPPRESS_SEQUENCE_TOKENS:
+        raise ValueError(f"at most {MAX_SUPPRESS_SEQUENCES} disabled ids, {MAX_SUPPRESS_SEQUENCES} suppressed sequences and "
+                         f"{MAX_SUPPRESS_SEQUENCE_TOKENS} suppressed tokens in all")
+    return penalty, int(no_repeat_ngram_size), ids, (offsets if len(offsets) > 1 else []), flat
+
+
+def _token_id(x, what: str, vocab_size: int) -> int:
+    if isinstance(x, (bool, np.bool_)) or not isinstance(x, (int, np.integer)):
+        raise ValueError(f"{what} must be an int, not {type(x).__name__}")
+    if not 0 <= x < vocab_size:
+        raise ValueError(f"{what} {x} is outside the target vocabulary [0, {vocab_size})")
+    return int(x)
 
 
 def _load_vocabulary(model_path: str, name: str) -> Optional[List[str]]:
@@ -163,9 +200,14 @@ class Translator:
                         num_hypotheses: int = 1, length_penalty: float = 1.0, max_decoding_length: int = 256,
                         min_decoding_length: int = 1, return_scores: bool = False, return_end_token: bool = False,
                         end_token: Union[None, str, Sequence[str], Sequence[int]] = None,
+                        repetition_penalty: float = 1, no_repeat_ngram_size: int = 0, disable_unk: bool = False,
+                        suppress_sequences: Optional[List[List[str]]] = None,
                         **unsupported) -> List[TranslationResult]:
         """source: list of token-string lists (looked up in the source vocabulary, special tokens added as the model asks)
-        or list of id lists (taken as they are)."""
+        or list of id lists (taken as they are).  The logits processors run on the device in every search step, on each
+        beam's tokens so far: repetition_penalty (> 0) rewrites them first, then no_repeat_ngram_size, disable_unk and
+        suppress_sequences (token strings of the target vocabulary; an unknown one raises ValueError, the unknown-token
+        string itself is accepted) disable tokens, as do the end tokens below min_decoding_length."""
         if target_prefix is not None and any(len(p) for p in target_prefix):
             raise ValueError("target_prefix is not supported by this engine")
         for k, v in unsupported.items():
@@ -176,6 +218,8 @@ class Translator:
                                  f"{_NEUTRAL[k]!r} only)")
         if max_decoding_length == 0 or min_decoding_length > max_decoding_length:
             raise ValueError("max_decoding_length must be > 0 and min_decoding_length must be <= max_decoding_length")
+        disable_ids, sequences = self._suppressed_ids(disable_unk, suppress_sequences)
+        _processor_options(repetition_penalty, no_repeat_ngram_size, disable_ids, sequences, self._tgt_vocab_size)
         rows = [list(r) for r in source]
         if not rows:
             return []
@@ -192,7 +236,9 @@ class Translator:
             ids, lens, scores = self.translate_ids(sub, beam_size=beam_size, patience=patience, num_hypotheses=num_hypotheses,
                                                    length_penalty=length_penalty, max_decoding_length=max_decoding_length,
                                                    min_decoding_length=min_decoding_length, return_end_token=return_end_token,
-                                                   end_token=end_token)
+                                                   end_token=end_token, repetition_penalty=repetition_penalty,
+                                                   no_repeat_ngram_size=no_repeat_ngram_size, disable_ids=disable_ids,
+                                                   suppress_sequences=sequences)
             for j, b in enumerate(keep):
                 hyp_ids = [ids[j, h, :lens[j, h]].tolist() for h in range(num_hypotheses) if lens[j, h] >= 0]
                 results[b] = TranslationResult([[self._target[i] for i in h] for h in hyp_ids], hyp_ids,
@@ -277,6 +323,34 @@ class Translator:
                 results[b] = ScoringResult([self._target_token(i) for i in tgt_rows[b][1 + offset:]], out[j, :n].tolist())
         return results
 
+    def _suppressed_ids(self, disable_unk, suppress_sequences):
+        """disable_unk and suppress_sequences as target ids (sequence_to_sequence.cc:341-362: Vocabulary::to_ids with
+        allow_unk = false).  The reference appends the unknown token to a vocabulary file that lacks it, past the output
+        layer: such an id is never produced, so there is nothing to disable and a sequence holding it never completes —
+        both are left out."""
+        if not isinstance(disable_unk, (bool, np.bool_)):
+            raise ValueError(f"disable_unk must be a bool, not {type(disable_unk).__name__}")
+        unk = self._tgt_to_id.get(self.unk_token, len(self._target))
+        disable = [unk] if disable_unk and unk < self._tgt_vocab_size else []
+        if suppress_sequences is None:
+            return disable, []
+        if isinstance(suppress_sequences, (str, bytes)) or not isinstance(suppress_sequences, (list, tuple)):
+            raise ValueError("suppress_sequences must be None or a list of token lists")
+        sequences = []
+        for seq in suppress_sequences:
+            if isinstance(seq, (str, bytes)) or not isinstance(seq, (list, tuple)):
+                raise ValueError("suppress_sequences must be None or a list of token lists")
+            ids = []
+            for tok in seq:
+                if not isinstance(tok, str):
+                    raise ValueError(f"suppress_sequences holds token strings, not {type(tok).__name__}")
+                if tok not in self._tgt_to_id and tok != self.unk_token:
+                    raise ValueError(f"Token {tok} is not in the vocabulary")
+                ids.append(self._tgt_to_id.get(tok, unk))
+            if all(i < self._tgt_vocab_size for i in ids):
+                sequences.append(ids)
+        return disable, sequences
+
     def _target_token(self, i: int) -> str:
         return self._target[i] if i < len(self._target) else self.unk_token
 
@@ -290,8 +364,12 @@ class Translator:
         return [int(e) for e in end_token]
 
     def translate_ids(self, rows, *, beam_size=2, patience=1.0, num_hypotheses=1, length_penalty=1.0, max_decoding_length=256,
-                      min_decoding_length=1, return_end_token=False, end_token=None, start_id: Optional[int] = None):
-        """ids in, ids out: (ids [batch, num_hypotheses, max_decoding_length], lens, scores [batch, num_hypotheses])."""
+                      min_decoding_length=1, return_end_token=False, end_token=None, start_id: Optional[int] = None,
+                      repetition_penalty=1.0, no_repeat_ngram_size=0, disable_ids=(), suppress_sequences=()):
+        """ids in, ids out: (ids [batch, num_hypotheses, max_decoding_length], lens, scores [batch, num_hypotheses]).
+        The logits processors take target ids: disable_ids are disabled at every step, suppress_sequences are id lists."""
+        penalty, ngram, disable_ids, seq_offsets, seq_ids = _processor_options(
+            repetition_penalty, no_repeat_ngram_size, disable_ids, suppress_sequences, self._tgt_vocab_size)
         B = len(rows)
         lens = np.array([len(r) for r in rows], np.int32)
         S = int(lens.max())
@@ -308,12 +386,20 @@ class Translator:
         out_lens = np.empty((B, num_hypotheses), np.int32)
         scores = np.zeros((B, num_hypotheses), np.float32)
         p = ctypes.c_void_p
-        check(lib().ct2b200_translate_batch(
-            p(self._h), src.ctypes.data_as(p), lens.ctypes.data_as(p), ctypes.c_int64(B), ctypes.c_int64(S), int(beam_size),
-            ctypes.c_float(patience), ctypes.c_float(length_penalty), ctypes.c_int64(max_decoding_length),
-            ctypes.c_int64(min_decoding_length), int(num_hypotheses), ctypes.c_int32(start_id), end_ids.ctypes.data_as(p),
-            int(end_ids.size), int(return_end_token), out.ctypes.data_as(p), out_lens.ctypes.data_as(p),
-            scores.ctypes.data_as(p)))
+        args = (p(self._h), src.ctypes.data_as(p), lens.ctypes.data_as(p), ctypes.c_int64(B), ctypes.c_int64(S), int(beam_size),
+                ctypes.c_float(patience), ctypes.c_float(length_penalty), ctypes.c_int64(max_decoding_length),
+                ctypes.c_int64(min_decoding_length), int(num_hypotheses), ctypes.c_int32(start_id), end_ids.ctypes.data_as(p),
+                int(end_ids.size), int(return_end_token))
+        outs = (out.ctypes.data_as(p), out_lens.ctypes.data_as(p), scores.ctypes.data_as(p))
+        if penalty == 1 and ngram == 0 and not disable_ids and not seq_offsets:
+            check(lib().ct2b200_translate_batch(*args, *outs))
+        else:
+            dis = np.array(disable_ids, np.int32)
+            offsets = np.array(seq_offsets, np.int32)
+            flat = np.array(seq_ids, np.int32)
+            check(lib().ct2b200_translate_batch_processors(
+                *args, ctypes.c_float(penalty), int(ngram), dis.ctypes.data_as(p), int(dis.size), flat.ctypes.data_as(p),
+                offsets.ctypes.data_as(p), max(0, int(offsets.size) - 1), *outs))
         return out, out_lens, scores
 
     def encode(self, rows) -> np.ndarray:

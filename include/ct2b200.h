@@ -414,6 +414,25 @@ CT2B200_API int ct2b200_translate_batch(ct2b200_translator* t, const int32_t* so
                             int64_t max_decoding_length, int64_t min_decoding_length, int num_hypotheses, int32_t start_id,
                             const int32_t* end_ids_h, int num_end_ids, int return_end_token, int32_t* out_ids_h,
                             int32_t* out_lens_h, float* out_scores_h);
+/* ct2b200_translate_batch with the logits processors of TranslationOptions (make_logits_processors, decoding.cc:1099-1112;
+ * RepetitionPenalty, NoRepeatNgram, SuppressTokens and SuppressSequences of src/decoding_utils.cc:40-177; disable_unk and
+ * suppress_sequences as SequenceToSequenceReplica::translate passes them, src/models/sequence_to_sequence.cc:341-362), applied
+ * on the device inside every search step, on each beam's history of chosen tokens.  The penalty rewrites the logits first;
+ * every disabled entry, the end ids below min_decoding_length included, is written last.
+ *   repetition_penalty > 0 and finite (1 = off); no_repeat_ngram_size >= 0 (0 = off);
+ *   disable_ids_h [num_disable_ids] target ids disabled at every step (disable_unk: the unknown-token id);
+ *   sequence_offsets_h [num_sequences + 1] (0 .. total) into sequence_ids_h [total]: a one-token sequence is disabled at every
+ *   step, the last token of a longer one when the history ends with the others, an empty one is ignored.
+ * Every id must lie inside the target vocabulary.  At most 4096 disabled ids, 4096 sequences and 65536 sequence tokens in all
+ * (the reference has no limit; larger tables are refused, not truncated).  With the processors off, the results are those of
+ * ct2b200_translate_batch. */
+CT2B200_API int ct2b200_translate_batch_processors(ct2b200_translator* t, const int32_t* source_ids_h,
+                            const int32_t* source_lens_h, int64_t batch, int64_t max_source_len, int beam_size, float patience,
+                            float length_penalty, int64_t max_decoding_length, int64_t min_decoding_length, int num_hypotheses,
+                            int32_t start_id, const int32_t* end_ids_h, int num_end_ids, int return_end_token,
+                            float repetition_penalty, int no_repeat_ngram_size, const int32_t* disable_ids_h, int num_disable_ids,
+                            const int32_t* sequence_ids_h, const int32_t* sequence_offsets_h, int num_sequences,
+                            int32_t* out_ids_h, int32_t* out_lens_h, float* out_scores_h);
 /* Host only (no device): the per-entry bookkeeping of one BeamSearch::search step (decoding.cc:595-663) — the SAME function the
  * device kernel runs (csrc/kernels/beam_decide.h).  words_h [2 * beam_size] = the candidates' tokens in TopK order.  Outputs:
  * active_h [beam] (candidate each next beam continues), hyp_slot_h / hyp_len_h [beam] (hypothesis registered for candidate k, or

@@ -334,6 +334,93 @@ def make_translator_score_fixture():
     print("translator score fixture:", sum(len(m["cases"]) for m in fixture["models"].values()), "cases")
 
 
+def ref_translate_processors(model_dir, compute, requests):
+    """Translator::translate_batch of the unmodified reference (CPU) with the logits processors, through
+    tools/ref_translate_processors.cc, built by tools/ref_translate_processors.mk against oracle/_ref/libct2ref.so into a
+    temporary directory.  requests: dicts of sources (token lists), beam_size, num_hypotheses, length_penalty, max_length,
+    min_length, repetition_penalty, no_repeat_ngram_size, disable_unk, suppress_sequences (token lists).  Per request: per
+    source (hypotheses as token lists, scores), or the reference's error message."""
+    import subprocess
+    import tempfile
+    out_dir = os.path.join(tempfile.gettempdir(), "ct2ref_processors")
+    subprocess.run(["make", "-s", "-f", "tools/ref_translate_processors.mk", "processors", "PROC_OUT=" + out_dir], cwd=ROOT,
+                   check=True)
+    lists = lambda ls: "|".join(" ".join(x) for x in ls)   # noqa: E731
+    text = "%s\t%s\n" % (model_dir, compute)
+    for r in requests:
+        text += "\t".join(str(x) for x in (r["beam_size"], r["num_hypotheses"], r["length_penalty"], r["max_length"],
+                                           r["min_length"], r["repetition_penalty"], r["no_repeat_ngram_size"],
+                                           int(r["disable_unk"]), lists(r["suppress_sequences"]), lists(r["sources"]))) + "\n"
+    lines = subprocess.run([os.path.join(out_dir, "ref_translate_processors")], input=text.encode(), capture_output=True,
+                           check=True).stdout.decode().split("\n")
+    res, k = [], 0
+    for r in requests:
+        if lines[k].startswith("ERROR\t"):
+            res.append(lines[k].split("\t", 1)[1])
+            k += 1
+            continue
+        entry = []
+        for _ in r["sources"]:
+            hyps, scores = lines[k].split("\t")
+            entry.append(([h.split(" ") if h else [] for h in hyps.split("|")], [float(x) for x in scores.split(" ")]))
+            k += 1
+        res.append(entry)
+    return res
+
+
+PROCESSOR_BEAMS = [(1, 1), (2, 2), (4, 3), (10, 2)]   # (beam, num_hypotheses); beam 10 takes the LogSoftMax + TopK path
+
+
+def processor_options(hyp, with_unk):
+    """The option sets of the processors fixture: each processor alone, then combinations.  `hyp` is a translation the
+    model makes without processors, so the suppressed sequences are ones it would produce."""
+    one, two, three = [hyp[0]], hyp[1:3], hyp[2:5]
+    opts = [dict(repetition_penalty=1.3), dict(repetition_penalty=0.7), dict(repetition_penalty=100.0),
+            dict(no_repeat_ngram_size=1), dict(no_repeat_ngram_size=2), dict(no_repeat_ngram_size=3),
+            dict(suppress_sequences=[one]), dict(suppress_sequences=[two]), dict(suppress_sequences=[three, []]),
+            dict(suppress_sequences=[one, two, three]),
+            dict(repetition_penalty=1.3, no_repeat_ngram_size=2, suppress_sequences=[two]),
+            dict(repetition_penalty=0.7, min_length=8),                    # the penalty lands before the min-length mask
+            dict(repetition_penalty=0.5, no_repeat_ngram_size=3, min_length=6, suppress_sequences=[one, three])]
+    if with_unk:                                    # the aren vocabularies have no <unk>: its id lies past the output layer
+        opts += [dict(disable_unk=True), dict(disable_unk=True, repetition_penalty=1.2, suppress_sequences=[["<unk>"], two])]
+    return opts
+
+
+def make_seq2seq_processors_fixture():
+    """Translator::translate_batch with repetition_penalty, no_repeat_ngram_size, disable_unk and suppress_sequences, from
+    the UNMODIFIED reference (oracle/_ref, CPU), on the models of seq2seq_ref.json (aren-transliteration-i8 and the post-norm
+    model) in float32 and int8: ragged batches of token strings, beams 1 / 2 / 4 / 10, each processor alone and combined."""
+    from ctranslate2_b200.translator import _load_vocabulary
+    fixture = {}
+    for name, mdir, lo, hi in (("aren", "aren-transliteration-i8", 4, 51), ("postnorm", "tiny_seq2seq_postnorm", 3, 120)):
+        path = os.path.join(OUT, mdir)
+        src_vocab = _load_vocabulary(path, "source_vocabulary")
+        entry = {"model": mdir, "models": {}}
+        for compute in ("float32", "int8"):
+            srcs = [[src_vocab[i] for i in r] for r in seq2seq_sources(300, 1, lo, hi)[0]]
+            srcs = (srcs + [[src_vocab[i] for i in r] for r in seq2seq_sources(301, 1, lo, hi)[0]])[:4]
+            plain = dict(sources=srcs, beam_size=2, num_hypotheses=1, length_penalty=1.0, max_length=20, min_length=1,
+                         repetition_penalty=1.0, no_repeat_ngram_size=0, disable_unk=False, suppress_sequences=[])
+            hyp = max((h[0][0] for h in ref_translate_processors(path, compute, [plain])[0]), key=len)
+            requests = []
+            for beam, nh in PROCESSOR_BEAMS:
+                for o in processor_options(hyp, name == "postnorm"):
+                    r = dict(plain, beam_size=beam, num_hypotheses=nh, max_length=16 if beam < 10 else 12)
+                    r.update(o)
+                    requests.append(r)
+            res = ref_translate_processors(path, compute, requests)
+            cases = []
+            for r, out in zip(requests, res):
+                assert not isinstance(out, str), out
+                cases.append(dict(r, hypotheses=[o[0] for o in out], scores=[o[1] for o in out]))
+            entry["models"][compute] = {"cases": cases}
+        fixture[name] = entry
+    with open(os.path.join(OUT, "seq2seq_processors_ref.json"), "w") as f:
+        json.dump(fixture, f, ensure_ascii=False)
+    print("seq2seq processors fixture:", sum(len(m["cases"]) for e in fixture.values() for m in e["models"].values()), "cases")
+
+
 WHISPER_CASES = [  # (beam, num_hypotheses, length_penalty, max_length, suppress_blank, timestamps)
     (1, 1, 1.0, 24, True, False), (3, 2, 1.0, 24, True, False), (5, 3, 1.0, 30, True, False), (5, 1, 0.0, 24, False, False),
     (2, 2, 0.7, 16, True, False), (1, 1, 1.0, 30, True, True), (5, 2, 1.0, 30, True, True), (3, 3, 1.0, 24, False, True)]
@@ -634,6 +721,9 @@ def main():
     if "--translator-score-only" in sys.argv:
         make_translator_score_fixture()
         return
+    if "--seq2seq-processors-only" in sys.argv:
+        make_seq2seq_processors_fixture()
+        return
     if "--processors-only" in sys.argv:
         make_processors_fixture()
         return
@@ -706,6 +796,7 @@ def main():
     make_score_fixture()
     make_seq2seq_fixture()
     make_translator_score_fixture()
+    make_seq2seq_processors_fixture()
     make_whisper_fixture()
     make_whisper_align_fixture()
     make_whisper_sampling_fixture()
