@@ -373,8 +373,11 @@ OPUS_MT_BASE = TransformerConfig(pre_norm=False, activation=2, start_from_zero_e
 
 
 def write_transformer_model(model_dir: str, cfg: TransformerConfig, quantization: str = "int8", seed: int = 1234,
-                            init_std: float = 0.05, emb_std: float = 0.3) -> None:
-    """Writes a random-init encoder-decoder Transformer directory (model.bin v6 + config.json + vocabularies)."""
+                            init_std: float = 0.05, emb_std: float = 0.3, alignment_layer: int = -1,
+                            alignment_heads: int = 1) -> None:
+    """Writes a random-init encoder-decoder Transformer directory (model.bin v6 + config.json + vocabularies).
+    alignment_layer / alignment_heads: the decoder's alignment attention (a negative layer counts from the end, 0 heads =
+    all of them); the defaults are the converters' own."""
     rng = np.random.default_rng(seed)
     is_int8 = quantization.startswith("int8")
     ftype = {"int8": "float32", "int8_float32": "float32", "int8_float16": "float16",
@@ -421,8 +424,8 @@ def write_transformer_model(model_dir: str, cfg: TransformerConfig, quantization
             w.add("encoder/embeddings_merge", np.int8(0))
             linear("encoder/embeddings_0", cfg.source_vocab, d, std=emb_std, bias=False)
         else:
-            w.add("decoder/alignment_layer", np.int16(-1))
-            w.add("decoder/alignment_heads", np.int16(1))
+            w.add("decoder/alignment_layer", np.int16(alignment_layer))
+            w.add("decoder/alignment_heads", np.int16(alignment_heads))
             w.add("decoder/alibi", np.int8(0))
             w.add("decoder/alibi_use_positive_positions", np.int8(0))
             w.add("decoder/scale_alibi", np.int8(0))

@@ -701,13 +701,14 @@ CT2B200_API int ct2b200_translate_batch(ct2b200_translator* t, const int32_t* so
   });
 }
 
-CT2B200_API int ct2b200_translate_batch_processors(ct2b200_translator* t, const int32_t* source_ids, const int32_t* source_lens,
+CT2B200_API int ct2b200_translate_batch_attention(ct2b200_translator* t, const int32_t* source_ids, const int32_t* source_lens,
                             int64_t batch, int64_t max_source_len, int beam_size, float patience, float length_penalty,
                             int64_t max_decoding_length, int64_t min_decoding_length, int num_hypotheses, int32_t start_id,
                             const int32_t* end_ids, int num_end_ids, int return_end_token, float repetition_penalty,
                             int no_repeat_ngram_size, const int32_t* disable_ids, int num_disable_ids,
-                            const int32_t* sequence_ids, const int32_t* sequence_offsets, int num_sequences, int32_t* out_ids,
-                            int32_t* out_lens, float* out_scores) {
+                            const int32_t* sequence_ids, const int32_t* sequence_offsets, int num_sequences,
+                            float coverage_penalty, int32_t* out_ids, int32_t* out_lens, float* out_scores,
+                            float* out_attention) {
   return guarded([&] {
     CT2_REQUIRE(t && source_ids && source_lens && out_ids && out_lens && out_scores, "translate_batch: null argument");
     CT2_REQUIRE(num_disable_ids >= 0 && num_sequences >= 0, "translate_batch: negative count");
@@ -727,8 +728,24 @@ CT2B200_API int ct2b200_translate_batch_processors(ct2b200_translator* t, const 
                   "suppress_sequences: at most 65536 tokens in all");
       r.sequence_ids.assign(sequence_ids, sequence_ids + total);
     }
+    r.coverage_penalty = coverage_penalty;
+    r.attention = out_attention;
     copy_hypotheses(t->impl->translate(r), batch, num_hypotheses, max_decoding_length, out_ids, out_lens, out_scores);
   });
+}
+
+CT2B200_API int ct2b200_translate_batch_processors(ct2b200_translator* t, const int32_t* source_ids, const int32_t* source_lens,
+                            int64_t batch, int64_t max_source_len, int beam_size, float patience, float length_penalty,
+                            int64_t max_decoding_length, int64_t min_decoding_length, int num_hypotheses, int32_t start_id,
+                            const int32_t* end_ids, int num_end_ids, int return_end_token, float repetition_penalty,
+                            int no_repeat_ngram_size, const int32_t* disable_ids, int num_disable_ids,
+                            const int32_t* sequence_ids, const int32_t* sequence_offsets, int num_sequences, int32_t* out_ids,
+                            int32_t* out_lens, float* out_scores) {
+  return ct2b200_translate_batch_attention(t, source_ids, source_lens, batch, max_source_len, beam_size, patience, length_penalty,
+                                           max_decoding_length, min_decoding_length, num_hypotheses, start_id, end_ids,
+                                           num_end_ids, return_end_token, repetition_penalty, no_repeat_ngram_size, disable_ids,
+                                           num_disable_ids, sequence_ids, sequence_offsets, num_sequences, 0.f, out_ids,
+                                           out_lens, out_scores, nullptr);
 }
 
 CT2B200_API int ct2b200_beam_decide_host(int beam_size, const int32_t* words, const int32_t* end_ids, int num_end_ids, int step,

@@ -116,6 +116,22 @@ void BeamSearchArena::set_processors(BeamState& bs, float repetition_penalty, in
   }
 }
 
+bool BeamSearchArena::ensure_attention(int64_t src_len, int heads) {
+  const int64_t N = cap_batch * cap_beam, hyps = cap_batch * max_hyp();
+  if (N <= attn_rows && cap_steps <= attn_steps && src_len <= attn_src && heads <= attn_heads && hyps <= attn_hyps) return false;
+  attn_rows = std::max(attn_rows, N);
+  attn_steps = std::max(attn_steps, cap_steps);
+  attn_src = std::max(attn_src, src_len);
+  attn_heads = std::max<int64_t>(attn_heads, heads);
+  attn_hyps = std::max(attn_hyps, hyps);
+  attn_probs.alloc(attn_rows * attn_heads * attn_src * 4);
+  attn_hist.alloc(attn_rows * attn_steps * attn_src * 4);
+  hyp_anc.alloc(attn_hyps * attn_steps * 4);
+  attn_cov.alloc(attn_hyps * 4);
+  attn_sel.alloc(attn_hyps * 4);
+  return true;
+}
+
 void BeamSearchArena::reset(const BeamState& bs, int32_t start_id, int dtype, cudaStream_t st) {
   CT2_CUDA_CHECK(cudaMemsetAsync(counters.ptr, 0, 64, st));
   CT2_CUDA_CHECK(cudaMemsetAsync(finished.ptr, 0, bs.batch * 4, st));
@@ -162,9 +178,18 @@ void BeamSearchArena::sample_step(void* logits, const BeamState& bs, int dtype, 
 
 // finalize_result (decoding.cc:189-254): normalise by length^penalty, sort (stable: equal scores keep registration order), keep
 // num_hypotheses, strip `strip_ids` from the tail
+// (decoding.cc:189-254), and finalize_hypothesis_score's coverage penalty (:176-203) when asked
 std::vector<TranslationHypotheses> BeamSearchArena::collect(const BeamState& bs, float length_penalty, int num_hypotheses,
-                                                            const std::vector<int32_t>& strip_ids, cudaStream_t st) {
+                                                            const std::vector<int32_t>& strip_ids, cudaStream_t st,
+                                                            float coverage_penalty, int S, float* attention, int64_t max_len) {
   const int64_t B = bs.batch, maxh = bs.max_hyp, stride = bs.stride;
+  CT2_REQUIRE((coverage_penalty == 0.f && !attention) || bs.hyp_anc, "collect: the search kept no attention");
+  std::vector<float> cov;
+  if (coverage_penalty != 0.f) {
+    cov.resize(B * maxh);
+    launch_hyp_coverage(bs, attn_hist.as<float>(), S, attn_cov.as<float>(), st);
+    CT2_CUDA_CHECK(cudaMemcpyAsync(cov.data(), attn_cov.ptr, B * maxh * 4, cudaMemcpyDeviceToHost, st));
+  }
   int32_t* h_nh = host;
   int32_t* h_len = h_nh + B;
   float* h_score = reinterpret_cast<float*>(h_len + B * maxh);
@@ -175,17 +200,20 @@ std::vector<TranslationHypotheses> BeamSearchArena::collect(const BeamState& bs,
   CT2_CUDA_CHECK(cudaMemcpyAsync(h_tok, hyp_tokens.ptr, B * maxh * stride * 4, cudaMemcpyDeviceToHost, st));
   CT2_CUDA_CHECK(cudaStreamSynchronize(st));
   std::vector<TranslationHypotheses> out(B);
+  std::vector<int32_t> sel(attention ? B * num_hypotheses : 0, -1);   // the returned slots, best first
   for (int64_t b = 0; b < B; ++b) {
     const int nh = h_nh[b];
     std::vector<float> sc(nh);
     for (int j = 0; j < nh; ++j) {
       const float len = static_cast<float>(h_len[b * maxh + j]);
       sc[j] = h_score[b * maxh + j] / std::pow(len, length_penalty);
+      if (coverage_penalty != 0.f) sc[j] += coverage_penalty * cov[b * maxh + j];
     }
     std::vector<int> order(nh);
     std::iota(order.begin(), order.end(), 0);
     std::stable_sort(order.begin(), order.end(), [&](int a, int c) { return sc[a] > sc[c]; });
     if (static_cast<int>(order.size()) > num_hypotheses) order.resize(num_hypotheses);
+    for (size_t k = 0; k < order.size() && attention; ++k) sel[b * num_hypotheses + k] = order[k];
     for (int j : order) {
       const int32_t* t = h_tok + (b * maxh + j) * stride;
       std::vector<int32_t> toks(t, t + h_len[b * maxh + j]);
@@ -193,6 +221,23 @@ std::vector<TranslationHypotheses> BeamSearchArena::collect(const BeamState& bs,
       out[b].tokens.push_back(std::move(toks));
       out[b].scores.push_back(sc[j]);
     }
+  }
+  if (attention) {
+    const size_t bytes = static_cast<size_t>(B) * num_hypotheses * max_len * S * 4;
+    if (bytes > attn_out.bytes) attn_out.alloc(bytes);
+    CT2_CUDA_CHECK(cudaMemcpyAsync(attn_sel.ptr, sel.data(), sel.size() * 4, cudaMemcpyHostToDevice, st));
+    launch_hyp_attention_gather(bs, attn_hist.as<float>(), S, attn_sel.as<int32_t>(), num_hypotheses, static_cast<int>(max_len),
+                                attn_out.as<float>(), st);
+    CT2_CUDA_CHECK(cudaMemcpyAsync(attention, attn_out.ptr, bytes, cudaMemcpyDeviceToHost, st));
+    CT2_CUDA_CHECK(cudaStreamSynchronize(st));
+    // the rows of stripped end tokens go with them (sequence_to_sequence.cc:383-391)
+    for (int64_t b = 0; b < B; ++b)
+      for (size_t k = 0; k < out[b].tokens.size(); ++k) {
+        const int32_t j = sel[b * num_hypotheses + k];
+        const int64_t kept = static_cast<int64_t>(out[b].tokens[k].size()), len = std::min<int64_t>(h_len[b * maxh + j], max_len);
+        if (len > kept)
+          std::memset(attention + ((b * num_hypotheses + static_cast<int64_t>(k)) * max_len + kept) * S, 0, (len - kept) * S * 4);
+      }
   }
   return out;
 }

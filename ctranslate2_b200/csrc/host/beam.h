@@ -22,6 +22,12 @@ struct BeamSearchArena {
   DeviceBuffer hyp_tokens, hyp_len, hyp_score;
   DeviceBuffer rng, sample_ids, sample_logp, row_score, row_done;   // sampled search
   DeviceBuffer processors;                // logits processors: [disabled ids | sequence offsets | sequence ids] int32
+  // the alignment attention, allocated by the first search that asks for it (return_attention, coverage_penalty): a step's
+  // per-head probabilities [N, heads, S] f32, the history [N, steps, S] f32 (row n, absolute position, source position),
+  // the hypotheses' ancestry [batch, max_hyp, steps]; at collect, the coverage terms [batch, max_hyp], the returned slots and
+  // their gathered rows
+  DeviceBuffer attn_probs, attn_hist, hyp_anc, attn_cov, attn_sel, attn_out;
+  int64_t attn_rows = 0, attn_steps = 0, attn_src = 0, attn_heads = 0, attn_hyps = 0;
   int32_t* host = nullptr;                // pinned staging of the results
   size_t host_elems = 0;
 
@@ -43,6 +49,9 @@ struct BeamSearchArena {
   // ensure_processors has sized, and points bs at them.
   void set_processors(BeamState& bs, float repetition_penalty, int no_repeat_ngram_size, const std::vector<int32_t>& disable_ids,
                       const std::vector<int32_t>& sequence_offsets, const std::vector<int32_t>& sequence_ids, cudaStream_t st);
+  // grows the attention buffers to the arena's capacities, `src_len` source positions and `heads` alignment heads; true when
+  // something was reallocated (captured graphs over them are stale then)
+  bool ensure_attention(int64_t src_len, int heads);
   // clears the counters / flags and starts every beam from start_id (beam 0 live, the others at the lowest score)
   void reset(const BeamState& bs, int32_t start_id, int dtype, cudaStream_t st);
   // one search step over logits [batch * beam, vocab] T (modified in place): log-probabilities + cumulative scores,
@@ -53,8 +62,12 @@ struct BeamSearchArena {
   void reset_sampling(BeamState& bs, int topk, float temperature, cudaStream_t st);
   // one sampled step over logits [batch * beam, vocab] T (modified in place)
   void sample_step(void* logits, const BeamState& bs, int dtype, cudaStream_t st);
+  // finalize_result; with bs.hyp_anc set (a search that kept the attention history of S source positions): coverage_penalty
+  // adds beta * the coverage term before the sort, and attention (host, or null) gets [batch, num_hypotheses, max_len, S] f32,
+  // the rows of the returned hypotheses (one per returned token), zeros past them
   std::vector<TranslationHypotheses> collect(const BeamState& bs, float length_penalty, int num_hypotheses,
-                                             const std::vector<int32_t>& strip_ids, cudaStream_t st);
+                                             const std::vector<int32_t>& strip_ids, cudaStream_t st, float coverage_penalty = 0.f,
+                                             int S = 0, float* attention = nullptr, int64_t max_len = 0);
 };
 
 // The process-wide random state of sampling (set_random_seed, src/random.cc): a seed, drawn once from std::random_device

@@ -119,6 +119,17 @@ Seq2SeqConfig parse_seq2seq_config(const ModelFile& f) {
       throw std::invalid_argument("embeddings_merge other than CONCAT of one feature is not supported");
   }
   mc.start_from_zero_embedding = f.attribute("decoder/start_from_zero_embedding", 0.0) != 0.0;
+  if (!mc.whisper) {
+    // TransformerDecoder (transformer.cc:518-528): a negative layer counts from the end, 0 heads = every head
+    int layer = static_cast<int>(scoped_attribute(f, "decoder", "alignment_layer", -1.0));
+    int heads = static_cast<int>(scoped_attribute(f, "decoder", "alignment_heads", 1.0));
+    if (layer < 0) layer += mc.dec_layers;
+    if (heads == 0) heads = mc.num_heads;
+    CT2_REQUIRE(layer >= 0 && layer < mc.dec_layers, "decoder/alignment_layer is outside the decoder's layers");
+    CT2_REQUIRE(heads >= 1 && heads <= mc.num_heads, "decoder/alignment_heads must be in [0, num_heads]");
+    mc.align_layer = layer;
+    mc.align_heads = heads;
+  }
   absent("decoder/scale_outputs", "scaled outputs");
   absent("decoder/layer_0/layer_scalar", "layer_scalar");
   absent("decoder/layer_0/self_attention/queries_scale", "a custom queries_scale");
@@ -488,7 +499,7 @@ void Translator::project_memory(int64_t batch, int64_t S) {
 // TransformerDecoder::decode's layer loop (transformer.cc:621-871), shared by the one-token step and the teacher-forced pass:
 // only the self-attention differs.  Cross-attention: row n reads memory entry n / rows_per_entry.
 bool Translator::run_decoder_layers(int64_t rows, int rows_per_entry, int64_t S, const std::function<void(int)>& self_attention,
-                                    const std::vector<AttnCapture>* capture) {
+                                    const std::vector<AttnCapture>* capture, bool align) {
   const float scale = 1.f / std::sqrt(static_cast<float>(mc_.head_dim));
   const bool pre = mc_.dec_pre_norm;
   bool xq = false;                                 // xq_ / xs_ already hold Quantize(x_) (left by a post-norm launch)
@@ -499,7 +510,14 @@ bool Translator::run_decoder_layers(int64_t rows, int rows_per_entry, int64_t S,
     dense(w.self.out, nullptr, ctx_.ptr, rows, x_.ptr, -1, x_.ptr);
     xq = !pre && post_norm(w.self.norm, x_.ptr, rows, &w.cross.in);
     dense(w.cross.in, pre ? &w.cross.norm : nullptr, x_.ptr, rows, nullptr, -1, q_.ptr, xq);
-    if (capture && (*capture)[l].masks)
+    if (align && l == mc_.align_layer) {
+      launch_attention_cross_align(q_.ptr, mem_kv_[l].ptr, src_lens_.as<int32_t>(), rows, rows_per_entry, static_cast<int>(S),
+                                   mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, beam_.attn_probs.as<float>(), mc_.align_heads,
+                                   dtype_, stream());
+      launch_align_mean(beam_.attn_probs.as<float>(), src_lens_.as<int32_t>(), beam_.counters.as<int32_t>(), rows, rows_per_entry,
+                        static_cast<int>(S), mc_.align_heads, static_cast<int>(beam_.cap_steps), beam_.attn_hist.as<float>(),
+                        dtype_, stream());
+    } else if (capture && (*capture)[l].masks)
       launch_attention_cross_capture(q_.ptr, mem_kv_[l].ptr, src_lens_.as<int32_t>(), rows, rows_per_entry, static_cast<int>(S),
                                      mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, (*capture)[l], dtype_, stream());
     else
@@ -523,7 +541,7 @@ void Translator::embed_decoder(const int32_t* ids_d, int64_t rows, int64_t time,
 }
 
 // TransformerDecoder::decode for one target position of every beam row (transformer.cc:621-871)
-void Translator::decoder_step(int64_t rows, int beam, int64_t batch, int64_t S) {
+void Translator::decoder_step(int64_t rows, int beam, int64_t batch, int64_t S, bool align) {
   (void)batch;
   const float scale = 1.f / std::sqrt(static_cast<float>(mc_.head_dim));
   const int32_t* step_ptr = beam_.counters.as<int32_t>();
@@ -531,14 +549,14 @@ void Translator::decoder_step(int64_t rows, int beam, int64_t batch, int64_t S) 
   const bool xq = run_decoder_layers(rows, beam, S, [&](int l) {
     launch_attention_beam_self(qkv_.ptr, self_k_[l].ptr, self_v_[l].ptr, beam_.anc.as<int32_t>(), step_ptr, rows,
                                static_cast<int>(cap_steps_), mc_.num_heads, mc_.head_dim, scale, ctx_.ptr, dtype_, stream());
-  });
+  }, nullptr, align);
   dense(projection_, mc_.has_dec_final_norm ? &dec_norm_ : nullptr, x_.ptr, rows, nullptr, -1, logits_.ptr, xq, logits_ld_);
 }
 
 void Translator::launch_or_capture_step(const BeamState& bs, int64_t S, const std::vector<int64_t>& key) {
   const int64_t rows = static_cast<int64_t>(bs.batch) * bs.beam;
   auto step = [&] {
-    decoder_step(rows, bs.beam, bs.batch, S);
+    decoder_step(rows, bs.beam, bs.batch, S, bs.hyp_anc != nullptr);
     if (bs.sample_topk >= 0)
       beam_.sample_step(logits_.ptr, bs, dtype_, stream());
     else
@@ -564,7 +582,8 @@ void Translator::run_search(const BeamState& bs, int64_t S, int64_t first_check)
   std::vector<int64_t> key = {bs.batch, bs.beam, S, bs.vocab_ld, bs.stride, bs.max_steps, bs.min_length, bs.max_hyp, bs.max_candidates,
                               bs.num_hypotheses, bs.early_exit, bs.num_end, bs.start_step, bs.include_eos, bs.num_disable,
                               bs.num_begin, bs.ts_begin, bs.ts_end, bs.ts_eot, bs.ts_no_timestamps, bs.ts_max_initial,
-                              bs.sample_topk, temperature_bits, penalty_bits, bs.no_repeat_ngram, bs.num_sequences};
+                              bs.sample_topk, temperature_bits, penalty_bits, bs.no_repeat_ngram, bs.num_sequences,
+                              bs.hyp_anc != nullptr};
   const int64_t poll = eos_poll_interval();
   int32_t* hfin = beam_.host;
   for (int64_t s = 0; s < bs.max_steps; ++s) {
@@ -614,7 +633,10 @@ std::vector<TranslationHypotheses> Translator::translate(const TranslationReques
     CT2_REQUIRE(r.sequence_offsets[s] <= r.sequence_offsets[s + 1], "suppress_sequences: offsets must not decrease");
   for (const std::vector<int32_t>* ids : {&r.disable_ids, &r.sequence_ids})
     for (int32_t id : *ids) CT2_REQUIRE(id >= 0 && id < mc_.tgt_vocab, "suppressed token id outside the target vocabulary");
+  CT2_REQUIRE(std::isfinite(r.coverage_penalty), "coverage_penalty must be finite");
+  const bool keep_attention = r.attention || r.coverage_penalty != 0.f;
   ensure_arena(B, S, beam, L);
+  if (keep_attention && beam_.ensure_attention(S, mc_.align_heads)) drop_graph();   // the step reads them through their address
   const size_t table = r.disable_ids.size() + r.sequence_offsets.size() + r.sequence_ids.size();
   if (table * 4 > beam_.processors.bytes) drop_graph();          // the captured step reads the tables through their address
   beam_.ensure_processors(table);
@@ -642,9 +664,12 @@ std::vector<TranslationHypotheses> Translator::translate(const TranslationReques
   set_logits_ld(bs);
   beam_.set_processors(bs, r.repetition_penalty, r.no_repeat_ngram_size, r.disable_ids, r.sequence_offsets, r.sequence_ids,
                        stream());
+  if (keep_attention) bs.hyp_anc = beam_.hyp_anc.as<int32_t>();
+  if (r.coverage_penalty != 0.f) bs.early_exit = 0;               // decoding.cc:457: no early exit under a coverage penalty
   beam_.reset(bs, r.start_id, dtype_, stream());
   run_search(bs, S, std::max<int64_t>(0, r.min_decoding_length));
-  return beam_.collect(bs, r.length_penalty, r.num_hypotheses, r.return_end_token ? std::vector<int32_t>{} : r.end_ids, stream());
+  return beam_.collect(bs, r.length_penalty, r.num_hypotheses, r.return_end_token ? std::vector<int32_t>{} : r.end_ids, stream(),
+                       r.coverage_penalty, static_cast<int>(S), r.attention, L);
 }
 
 // =============================================================================================

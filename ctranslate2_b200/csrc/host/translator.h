@@ -25,6 +25,9 @@ struct Seq2SeqConfig {
   bool round_before_cast = true;                     // binary version >= 5 (model.h:87-89)
   bool has_enc_final_norm = false, has_dec_final_norm = false;
   bool start_from_zero_embedding = false;            // Marian / OPUS-MT decoders (transformer.cc:637-640)
+  // the alignment attention a Translator returns (transformer.cc:518-528): the mean of the normalised cross-attention of
+  // heads [0, align_heads) of decoder layer align_layer (the attributes' defaults: the last layer, one head)
+  int align_layer = 0, align_heads = 1;
   bool whisper = false;                              // WhisperSpec: Conv1D front-end instead of source embeddings
   int64_t n_mels = 0, max_frames = 0;                // Whisper: input channels, encoder positions (frames / 2)
   // TransformerEncoderSpec (models::EncoderReplica, language_model.cc:302-400): the encoder alone, no decoder
@@ -81,6 +84,9 @@ struct TranslationRequest {
   std::vector<int32_t> disable_ids;       // SuppressTokens (disable_unk: the target vocabulary's unknown-token id)
   std::vector<int32_t> sequence_offsets;  // SuppressSequences: sequence s = sequence_ids[offsets[s] .. offsets[s + 1]);
   std::vector<int32_t> sequence_ids;      //   no offsets = no sequences
+  // the alignment attention, kept on the device for every beam when either is asked (decoding.cc:176-254, 425-720)
+  float coverage_penalty = 0.f;           // beta of the GNMT coverage term added at finalize (finite; 0 = off)
+  float* attention = nullptr;             // host [batch, num_hypotheses, max_decoding_length, max_source_len] f32, or null
 };
 // The reference takes any number of suppressed sequences; this engine refuses more than these, never truncates.
 constexpr int64_t kMaxSuppressSequences = 4096;      // sequences, and disabled ids
@@ -203,8 +209,9 @@ class Translator {
   // the decoder layer stack on `rows` rows of x_; `self_attention(layer)` fills ctx_ from qkv_, and each run of
   // `rows_per_entry` rows attends to one memory entry.  Returns whether xq_ / xs_ hold Quantize(x_).
   // `capture` (one entry per layer, count 0 = none): the cross-attention also saves the scores of those heads
+  // `align`: the alignment layer's cross-attention also writes the step's row of beam_'s attention history
   bool run_decoder_layers(int64_t rows, int rows_per_entry, int64_t S, const std::function<void(int)>& self_attention,
-                          const std::vector<AttnCapture>* capture = nullptr);
+                          const std::vector<AttnCapture>* capture = nullptr, bool align = false);
   // the teacher-forced pass of score / whisper_align / whisper_detect_language: `entries` sequences of T decoder inputs ids_d
   // [entries * T] at positions 0 .. T - 1 with causal self-attention, each attending to its memory entry of S positions.
   // Returns whether xq_ / xs_ hold Quantize(x_).
@@ -219,7 +226,8 @@ class Translator {
   int64_t ensure_score_slab();
   // copies `ids` into score_ids_ (grown as needed); `ids` must stay alive until the copy is done
   const int32_t* stage_ids(const std::vector<int32_t>& ids);
-  void decoder_step(int64_t rows, int beam, int64_t batch, int64_t S);
+  // align: keep the step's alignment attention (a search with bs.hyp_anc set)
+  void decoder_step(int64_t rows, int beam, int64_t batch, int64_t S, bool align = false);
   // one decoding step, captured as the graph of `key` (everything the capture bakes in) unless use_graph_ is off
   void launch_or_capture_step(const BeamState& bs, int64_t S, const std::vector<int64_t>& key);
 

@@ -195,6 +195,15 @@ struct AttnCapture {
 };
 void launch_attention_cross_capture(const void* q, const void* kv, const int32_t* lengths, int64_t rows, int beam, int S, int H,
                                     int D, float scale, void* out, const AttnCapture& cap, int dtype, cudaStream_t st);
+// The same cross-attention, also writing the normalised probabilities of heads [0, heads) (what a Translator decoder returns,
+// return_normalized_attention() == true) to probs [rows, heads, S] f32; keys past a row's entry length are not written.
+void launch_attention_cross_align(const void* q, const void* kv, const int32_t* lengths, int64_t rows, int beam, int S, int H,
+                                  int D, float scale, void* out, float* probs, int heads, int dtype, cudaStream_t st);
+// the alignment attention of one decoding step (TransformerDecoder::decode, transformer.cc:811-838, averaged heads): row n of
+// the history hist [rows, stride, S] f32 at position *step_ptr = T(the mean of probs [n, 0 .. heads, s]), summed in head
+// order; exact zeros past the length of entry n / beam
+void launch_align_mean(const float* probs, const int32_t* lengths, const int32_t* step_ptr, int64_t rows, int beam, int S,
+                       int heads, int stride, float* hist, int dtype, cudaStream_t st);
 // causal self-attention of `time` teacher-forced decoder positions per sequence: qkv [batch * time, 3d] (row b * time + t
 // attends to rows b * time + j, j <= t), out [batch * time, d]; no cache is written
 void launch_attention_causal(const void* qkv, int64_t batch, int time, int H, int D, float scale, void* out, int dtype,
@@ -231,6 +240,9 @@ struct BeamState {
   int32_t* hyp_tokens = nullptr;    // [batch, max_hyp, stride]
   int32_t* hyp_len = nullptr;       // [batch, max_hyp]
   float* hyp_score = nullptr;       // [batch, max_hyp] cumulative log-probability (not normalised)
+  // [batch, max_hyp, stride] or null: the cache slot that computed each absolute position of a hypothesis, filled when it is
+  // registered (its attention row t is then row hyp_anc[t] of the history at position t)
+  int32_t* hyp_anc = nullptr;
   // Sampled search (GreedySearch with a RandomSampler, decoding.cc:751-971): sample_topk >= 0 selects it.  The `beam` rows of an
   // entry are its num_hypotheses independent samples; ancestry stays the identity and hypothesis slot h belongs to row h.
   int sample_topk = -1;             // 0 = the whole vocabulary
@@ -253,6 +265,13 @@ void launch_beam_force(const BeamState& s, const int32_t* forced_next, cudaStrea
 // -> s.sample_ids / s.sample_logp, then the update: histories, row scores, hypothesis h of a row that ends, step + 1
 void launch_beam_sample(void* logits, const BeamState& s, int dtype, cudaStream_t st);
 void launch_beam_sample_update(const BeamState& s, cudaStream_t st);
+// compute_coverage_penalty (decoding.cc:176-187) without its factor, for every registered hypothesis (s.hyp_anc set) over the
+// attention history hist [N, s.stride, S]: out [batch, max_hyp] f32 (slots past num_hyp untouched)
+void launch_hyp_coverage(const BeamState& s, const float* hist, int S, float* out, cudaStream_t st);
+// out [batch, num, max_len, S] f32 = the attention rows of hypothesis slot sel[b * num + k] (device, -1 = none) of entry b,
+// zeros past its length
+void launch_hyp_attention_gather(const BeamState& s, const float* hist, int S, const int32_t* sel, int num, int max_len,
+                                 float* out, cudaStream_t st);
 // RandomSampler::sample on rows x [rows, ld] T of `vocab` logits: ids [rows], logp [rows] = T(LogSoftMax(x))[id]; the
 // uniform of row r is philox_uniform(seed, call, r, step) (philox.h)
 void launch_random_sample(const void* x, int64_t rows, int64_t vocab, int64_t ld, int k, float temperature, uint32_t seed,

@@ -203,17 +203,26 @@ struct AttnGeneric {
   bool vec_ok;               // every row start (q, k, v, caches, out) is 16-byte aligned
 };
 
-// the capture argument of the CAP instantiations; the others take an empty one, so their parameter block keeps its size
+// The extra output of an instantiation and its argument: none (an empty one, so the parameter block keeps its size), the
+// pre-softmax scores of selected heads (kCapture: Whisper::align) or the normalised probabilities of the alignment heads
+// (kAlign: the attention a Translator returns, launch_attention_cross_align).
+enum AttnExtra { kNoExtra = 0, kCapture = 1, kAlign = 2 };
 struct NoCapture {};
-template <bool CAP> using CaptureArg = std::conditional_t<CAP, AttnCapture, NoCapture>;
+struct AttnAlign {
+  float* probs;              // [rows, heads, S]
+  int heads;
+};
+template <int X>
+using ExtraArg = std::conditional_t<X == kCapture, AttnCapture, std::conditional_t<X == kAlign, AttnAlign, NoCapture>>;
 
 constexpr int kAttnWarps = 4;
 
 // DT = head_dim known at compile time (64, 128: the loops over a key / value row unroll, so the 16-byte loads of a row are all
-// in flight at once — with a run-time bound they are issued one L2 round trip at a time), 0 = any head_dim.  CAP: also write
-// the scores of the heads a.cap selects (Whisper::align); the other instantiations compile without it.
-template <typename T, int MODE, int DT, bool CAP = false>
-__global__ void __launch_bounds__(kAttnWarps * 32) attention_generic_kernel(AttnGeneric a, CaptureArg<CAP> cap) {
+// in flight at once — with a run-time bound they are issued one L2 round trip at a time), 0 = any head_dim.  X = kCapture: also
+// write the scores of the heads cap selects (Whisper::align); X = kAlign: also write the probabilities of heads
+// [0, cap.heads); the other instantiations compile without either.
+template <typename T, int MODE, int DT, int X = kNoExtra>
+__global__ void __launch_bounds__(kAttnWarps * 32) attention_generic_kernel(AttnGeneric a, ExtraArg<X> cap) {
   extern __shared__ float smem_f[];
   griddep_launch();
   griddep_wait();
@@ -295,7 +304,7 @@ __global__ void __launch_bounds__(kAttnWarps * 32) attention_generic_kernel(Attn
     return dot;
   };
   uint32_t cap_mask = 0;     // CAP: the slots this head is saved to, read once per warp
-  if constexpr (CAP) cap_mask = cap.masks[h];
+  if constexpr (X == kCapture) cap_mask = cap.masks[h];
   // scores: one key per lane
   float m = -INFINITY;
   for (int j = lane; j < nkeys; j += 32) {
@@ -308,7 +317,7 @@ __global__ void __launch_bounds__(kAttnWarps * 32) attention_generic_kernel(Attn
     const float s = round_to<T>(dot * a.scale);
     sc[j] = s;
     m = fmaxf(m, s);
-    if constexpr (CAP) {
+    if constexpr (X == kCapture) {
       const int64_t e = n / a.beam, t = n - e * a.beam;
       for (uint32_t mk = cap_mask; mk; mk &= mk - 1)
         cap.out[((e * cap.total + cap.first + __ffs(mk) - 1) * a.beam + t) * a.S + j] = s;
@@ -318,7 +327,12 @@ __global__ void __launch_bounds__(kAttnWarps * 32) attention_generic_kernel(Attn
   float sum = 0.f;
   for (int j = lane; j < nkeys; j += 32) sum += expf(sc[j] - m);
   sum = warp_sum(sum);
-  for (int j = lane; j < nkeys; j += 32) sc[j] = round_to<T>(expf(sc[j] - m) / sum);
+  for (int j = lane; j < nkeys; j += 32) {
+    sc[j] = round_to<T>(expf(sc[j] - m) / sum);
+    if constexpr (X == kAlign) {
+      if (h < cap.heads) cap.probs[(n * cap.heads + h) * a.S + j] = sc[j];
+    }
+  }
   __syncwarp();
   T* orow = static_cast<T*>(a.out) + n * a.out_stride + h * D;
   auto value_row = [&](int j) -> const T* {
@@ -744,6 +758,13 @@ __global__ void __launch_bounds__(128) beam_update_kernel(BeamState st, const T*
     const int32_t* src = alive_r + static_cast<int64_t>(i * beam + s_origin[k]) * L;
     for (int t = threadIdx.x; t < rel; t += blockDim.x) dst[t] = src[t];
     if (threadIdx.x == 0) dst[rel] = s_word[k];
+    if (st.hyp_anc) {
+      // the slots that computed its positions: the origin beam's ancestry, then the origin row itself
+      int32_t* da = st.hyp_anc + (static_cast<int64_t>(i) * st.max_hyp + slot) * L;
+      const int32_t* sa = anc_r + static_cast<int64_t>(i * beam + s_origin[k]) * L;
+      for (int t = threadIdx.x; t < step; t += blockDim.x) da[t] = sa[t];
+      if (threadIdx.x == 0) da[step] = i * beam + s_origin[k];
+    }
   }
   // the next beams
   for (int k = 0; k < beam; ++k) {
@@ -1014,8 +1035,8 @@ void launch_layer_norm(const void* x, const void* gamma, const void* beta, int64
 }
 
 namespace {
-template <typename T, int MODE, bool CAP = false>
-void launch_attn_mode(const AttnGeneric& a_in, cudaStream_t st, const CaptureArg<CAP>& cap = {}) {
+template <typename T, int MODE, int X = kNoExtra>
+void launch_attn_mode(const AttnGeneric& a_in, cudaStream_t st, const ExtraArg<X>& cap = {}) {
   AttnGeneric a = a_in;
   {
     const size_t es = sizeof(T);
@@ -1025,8 +1046,8 @@ void launch_attn_mode(const AttnGeneric& a_in, cudaStream_t st, const CaptureArg
   }
   const size_t smem = static_cast<size_t>(kAttnWarps) * (a.max_keys + a.D) * sizeof(float);
   CT2_REQUIRE(smem <= 200 * 1024, "attention: too many keys for the generic kernel");
-  auto kernel = a.D == 64 ? attention_generic_kernel<T, MODE, 64, CAP>
-                : a.D == 128 ? attention_generic_kernel<T, MODE, 128, CAP> : attention_generic_kernel<T, MODE, 0, CAP>;
+  auto kernel = a.D == 64 ? attention_generic_kernel<T, MODE, 64, X>
+                : a.D == 128 ? attention_generic_kernel<T, MODE, 128, X> : attention_generic_kernel<T, MODE, 0, X>;
   if (smem > 48 * 1024) {
     // the attribute is per device: set it whenever the request grows (cheap, idempotent)
     CT2_CUDA_CHECK(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
@@ -1154,7 +1175,117 @@ void launch_attention_cross_capture(const void* q, const void* kv, const int32_t
   a.D = D;
   a.scale = scale;
   a.max_keys = S;
-  CT2_DISPATCH_DTYPE(dtype, (launch_attn_mode<T, 2, true>(a, st, cap)));
+  CT2_DISPATCH_DTYPE(dtype, (launch_attn_mode<T, 2, kCapture>(a, st, cap)));
+}
+
+void launch_attention_cross_align(const void* q, const void* kv, const int32_t* lengths, int64_t rows, int beam, int S, int H,
+                                  int D, float scale, void* out, float* probs, int heads, int dtype, cudaStream_t st) {
+  if (rows == 0) return;
+  CT2_REQUIRE(probs && heads >= 1 && heads <= H, "attention alignment: bad heads");
+  const int64_t d = static_cast<int64_t>(H) * D;
+  const size_t es = dtype_size(dtype);
+  AttnGeneric a{};
+  a.q = q;
+  a.q_stride = d;
+  a.k = kv;
+  a.v = static_cast<const uint8_t*>(kv) + d * es;
+  a.kv_stride = 2 * d;
+  a.out = out;
+  a.out_stride = d;
+  a.lengths = lengths;
+  a.rows = rows;
+  a.S = S;
+  a.beam = beam;
+  a.H = H;
+  a.D = D;
+  a.scale = scale;
+  a.max_keys = S;
+  const AttnAlign al{probs, heads};
+  CT2_DISPATCH_DTYPE(dtype, (launch_attn_mode<T, 2, kAlign>(a, st, al)));
+}
+
+namespace {
+// ops::Mean over the alignment heads (transformer.cc:826-829) of one decoding step, in a fixed head order: row n's entry of
+// the attention history at the device-resident step; positions past the entry's length are exact zeros.
+template <typename T>
+__global__ void __launch_bounds__(128) align_mean_kernel(const float* __restrict__ probs, const int32_t* __restrict__ lengths,
+                                                         const int32_t* __restrict__ step_ptr, int beam, int S, int heads,
+                                                         int stride, float* __restrict__ hist) {
+  griddep_launch();
+  griddep_wait();
+  const int64_t n = blockIdx.x;
+  const int len = min(lengths[n / beam], S);
+  float* out = hist + (n * stride + *step_ptr) * S;
+  const float* p = probs + n * heads * S;
+  for (int s = threadIdx.x; s < S; s += blockDim.x) {
+    float v = 0.f;
+    if (s < len) {
+      for (int h = 0; h < heads; ++h) v += p[h * S + s];
+      v = round_to<T>(v / static_cast<float>(heads));
+    }
+    out[s] = v;
+  }
+}
+
+// The coverage term of compute_coverage_penalty (decoding.cc:176-187) of every registered hypothesis, one CTA per (entry,
+// slot): sum over the columns with coverage > 0 of log(min(coverage, 1)), coverage = the column summed over the hypothesis's
+// rows in order; beta is applied by the caller.
+__global__ void __launch_bounds__(128) hyp_coverage_kernel(BeamState st, const float* __restrict__ hist, int S,
+                                                           float* __restrict__ out) {
+  __shared__ float red[32];
+  const int i = blockIdx.x, j = blockIdx.y;
+  if (j >= st.num_hyp[i]) return;
+  const int64_t h = static_cast<int64_t>(i) * st.max_hyp + j;
+  const int len = st.hyp_len[h];
+  const int32_t* anc = st.hyp_anc + h * st.stride;
+  float pen = 0.f;
+  for (int s = threadIdx.x; s < S; s += blockDim.x) {
+    float cov = 0.f;
+    for (int t = 0; t < len; ++t) cov += hist[(static_cast<int64_t>(anc[t]) * st.stride + t) * S + s];
+    if (cov > 0.f) pen += logf(fminf(cov, 1.f));
+  }
+  pen = block_reduce<false>(pen, red);
+  if (threadIdx.x == 0) out[h] = pen;
+}
+
+// out [batch, num, max_len, S]: the attention rows of hypothesis slot sel[b * num + k] of entry b (-1: none), zeros past its
+// length
+__global__ void __launch_bounds__(128) hyp_attention_gather_kernel(BeamState st, const float* __restrict__ hist, int S,
+                                                                   const int32_t* __restrict__ sel, int num, int max_len,
+                                                                   float* __restrict__ out) {
+  const int b = blockIdx.x / num;
+  const int slot = sel[blockIdx.x];
+  const int64_t h = static_cast<int64_t>(b) * st.max_hyp + slot;
+  const int len = slot >= 0 ? min(st.hyp_len[h], max_len) : 0;
+  float* o = out + static_cast<int64_t>(blockIdx.x) * max_len * S;
+  for (int64_t e = threadIdx.x; e < static_cast<int64_t>(max_len) * S; e += blockDim.x) {
+    const int t = static_cast<int>(e / S), s = static_cast<int>(e % S);
+    o[e] = t < len ? hist[(static_cast<int64_t>(st.hyp_anc[h * st.stride + t]) * st.stride + t) * S + s] : 0.f;
+  }
+}
+}  // namespace
+
+void launch_align_mean(const float* probs, const int32_t* lengths, const int32_t* step_ptr, int64_t rows, int beam, int S,
+                       int heads, int stride, float* hist, int dtype, cudaStream_t st) {
+  if (rows == 0) return;
+  CT2_DISPATCH_DTYPE(dtype, (launch_pdl(align_mean_kernel<T>, dim3(static_cast<unsigned>(rows)), dim3(128), 0, st, probs, lengths,
+                                        step_ptr, beam, S, heads, stride, hist)));
+  check_launch();
+}
+
+void launch_hyp_coverage(const BeamState& s, const float* hist, int S, float* out, cudaStream_t st) {
+  if (s.batch == 0) return;
+  CT2_REQUIRE(s.hyp_anc, "hyp_coverage: no hypothesis ancestry");
+  hyp_coverage_kernel<<<dim3(s.batch, s.max_hyp), 128, 0, st>>>(s, hist, S, out);
+  check_launch();
+}
+
+void launch_hyp_attention_gather(const BeamState& s, const float* hist, int S, const int32_t* sel, int num, int max_len,
+                                 float* out, cudaStream_t st) {
+  if (s.batch == 0 || num == 0) return;
+  CT2_REQUIRE(s.hyp_anc, "hyp_attention_gather: no hypothesis ancestry");
+  hyp_attention_gather_kernel<<<s.batch * num, 128, 0, st>>>(s, hist, S, sel, num, max_len, out);
+  check_launch();
 }
 
 void launch_beam_init(void* cum, int32_t* ids, int64_t rows, int beam, int start_id, int dtype, cudaStream_t st) {

@@ -26,6 +26,7 @@ class TranslationResult:
     hypotheses: List[List[str]]
     hypotheses_ids: List[List[int]]
     scores: List[float] = field(default_factory=list)
+    attention: List[List[List[float]]] = field(default_factory=list)
 
 
 def translator_summary(model_path: str) -> dict:
@@ -37,9 +38,9 @@ def translator_summary(model_path: str) -> dict:
 
 # TranslationOptions (include/ctranslate2/translation.h:14-98) this engine does not implement, with the only value it accepts
 _NEUTRAL = {
-    "coverage_penalty": 0, "prefix_bias_beta": 0, "sampling_topk": 1, "sampling_topp": 1, "sampling_temperature": 1,
-    "use_vmap": False, "return_attention": False, "return_logits_vocab": False, "return_alternatives": False,
-    "min_alternative_expansion_prob": 0, "replace_unknowns": False, "callback": None, "asynchronous": False,
+    "prefix_bias_beta": 0, "sampling_topk": 1, "sampling_topp": 1, "sampling_temperature": 1,
+    "use_vmap": False, "return_logits_vocab": False, "return_alternatives": False,
+    "min_alternative_expansion_prob": 0, "callback": None, "asynchronous": False,
     "max_batch_size": 0, "batch_type": "examples", "max_input_length": 1024,
 }
 
@@ -86,12 +87,34 @@ def _processor_options(repetition_penalty, no_repeat_ngram_size, disable_ids, su
     return penalty, int(no_repeat_ngram_size), ids, (offsets if len(offsets) > 1 else []), flat
 
 
+def _coverage_penalty(coverage_penalty) -> float:
+    if isinstance(coverage_penalty, (bool, np.bool_)) or not isinstance(coverage_penalty, (int, float, np.integer, np.floating)):
+        raise ValueError(f"coverage_penalty must be a number, not {type(coverage_penalty).__name__}")
+    if not np.isfinite(float(coverage_penalty)):
+        raise ValueError(f"coverage_penalty must be finite, got {coverage_penalty!r}")
+    return float(coverage_penalty)
+
+
+def _flag(name: str, value) -> bool:
+    if not isinstance(value, (bool, np.bool_)):
+        raise ValueError(f"{name} must be a bool, not {type(value).__name__}")
+    return bool(value)
+
+
 def _token_id(x, what: str, vocab_size: int) -> int:
     if isinstance(x, (bool, np.bool_)) or not isinstance(x, (int, np.integer)):
         raise ValueError(f"{what} must be an int, not {type(x).__name__}")
     if not 0 <= x < vocab_size:
         raise ValueError(f"{what} {x} is outside the target vocabulary [0, {vocab_size})")
     return int(x)
+
+
+def _replace_unknowns(hypothesis: List[str], source: List[str], attention: np.ndarray, unk_token: str) -> None:
+    """replace_unknown_tokens (sequence_to_sequence.cc:288-302): each unknown token becomes the source token of its
+    attention row's first maximum."""
+    for t, token in enumerate(hypothesis):
+        if token == unk_token and source:
+            hypothesis[t] = source[int(np.argmax(attention[t]))]
 
 
 def _load_vocabulary(model_path: str, name: str) -> Optional[List[str]]:
@@ -201,13 +224,24 @@ class Translator:
                         min_decoding_length: int = 1, return_scores: bool = False, return_end_token: bool = False,
                         end_token: Union[None, str, Sequence[str], Sequence[int]] = None,
                         repetition_penalty: float = 1, no_repeat_ngram_size: int = 0, disable_unk: bool = False,
-                        suppress_sequences: Optional[List[List[str]]] = None,
+                        suppress_sequences: Optional[List[List[str]]] = None, return_attention: bool = False,
+                        replace_unknowns: bool = False, coverage_penalty: float = 0,
                         **unsupported) -> List[TranslationResult]:
         """source: list of token-string lists (looked up in the source vocabulary, special tokens added as the model asks)
         or list of id lists (taken as they are).  The logits processors run on the device in every search step, on each
         beam's tokens so far: repetition_penalty (> 0) rewrites them first, then no_repeat_ngram_size, disable_unk and
         suppress_sequences (token strings of the target vocabulary; an unknown one raises ValueError, the unknown-token
-        string itself is accepted) disable tokens, as do the end tokens below min_decoding_length."""
+        string itself is accepted) disable tokens, as do the end tokens below min_decoding_length.
+
+        The search keeps the alignment attention of every beam on the device (the mean of the normalised cross-attention of
+        the model's alignment heads) when one of these asks for it:
+          * return_attention: TranslationResult.attention holds, per hypothesis, one row per token over the source tokens
+            (the special tokens the model adds are left out; sequence_to_sequence.cc:395-412);
+          * replace_unknowns: each unknown-token string of a hypothesis becomes the source token it attends to most (the
+            first of equal maxima).  Sources given as ids have no tokens to copy: ValueError (the reference has no id
+            input);
+          * coverage_penalty: the GNMT coverage term beta * sum(log(min(coverage, 1))) over the attended source positions
+            joins each hypothesis's final score before the hypotheses are ranked (decoding.cc:176-254)."""
         if target_prefix is not None and any(len(p) for p in target_prefix):
             raise ValueError("target_prefix is not supported by this engine")
         for k, v in unsupported.items():
@@ -220,30 +254,68 @@ class Translator:
             raise ValueError("max_decoding_length must be > 0 and min_decoding_length must be <= max_decoding_length")
         disable_ids, sequences = self._suppressed_ids(disable_unk, suppress_sequences)
         _processor_options(repetition_penalty, no_repeat_ngram_size, disable_ids, sequences, self._tgt_vocab_size)
-        rows = [list(r) for r in source]
-        if not rows:
+        return_attention = _flag("return_attention", return_attention)
+        replace_unknowns = _flag("replace_unknowns", replace_unknowns)
+        coverage_penalty = _coverage_penalty(coverage_penalty)
+        tokens = [list(r) for r in source]
+        is_text = [bool(r) and isinstance(r[0], str) for r in tokens]
+        if replace_unknowns and any(r and not t for r, t in zip(tokens, is_text)):
+            raise ValueError("replace_unknowns needs the source tokens: the sources were given as ids")
+        if not tokens:
             return []
-        rows = [self.source_ids(r) if (r and isinstance(r[0], str)) else [int(i) for i in r] for r in rows]
+        rows = [self.source_ids(r) if t else [int(i) for i in r] for r, t in zip(tokens, is_text)]
+        keep_attention = return_attention or replace_unknowns
         # an empty source (even with its special tokens) yields an empty translation (sequence_to_sequence.cc:288-303)
         keep = [b for b, r in enumerate(rows) if len(r) > 0]
         results: List[Optional[TranslationResult]] = [None] * len(rows)
         for b in range(len(rows)):
             if b not in keep:
                 results[b] = TranslationResult([[] for _ in range(num_hypotheses)], [[] for _ in range(num_hypotheses)],
-                                               [0.0] * num_hypotheses if return_scores else [])
+                                               [0.0] * num_hypotheses if return_scores else [],
+                                               [[] for _ in range(num_hypotheses)] if return_attention else [])
         if keep:
             sub = [rows[b] for b in keep]
-            ids, lens, scores = self.translate_ids(sub, beam_size=beam_size, patience=patience, num_hypotheses=num_hypotheses,
-                                                   length_penalty=length_penalty, max_decoding_length=max_decoding_length,
-                                                   min_decoding_length=min_decoding_length, return_end_token=return_end_token,
-                                                   end_token=end_token, repetition_penalty=repetition_penalty,
-                                                   no_repeat_ngram_size=no_repeat_ngram_size, disable_ids=disable_ids,
-                                                   suppress_sequences=sequences)
+            extra = dict(return_attention=True) if keep_attention else {}
+            if coverage_penalty != 0:
+                extra["coverage_penalty"] = coverage_penalty
+            out = self.translate_ids(sub, beam_size=beam_size, patience=patience, num_hypotheses=num_hypotheses,
+                                     length_penalty=length_penalty, max_decoding_length=max_decoding_length,
+                                     min_decoding_length=min_decoding_length, return_end_token=return_end_token,
+                                     end_token=end_token, repetition_penalty=repetition_penalty,
+                                     no_repeat_ngram_size=no_repeat_ngram_size, disable_ids=disable_ids,
+                                     suppress_sequences=sequences, **extra)
+            ids, lens, scores = out[:3]
             for j, b in enumerate(keep):
                 hyp_ids = [ids[j, h, :lens[j, h]].tolist() for h in range(num_hypotheses) if lens[j, h] >= 0]
-                results[b] = TranslationResult([[self._target[i] for i in h] for h in hyp_ids], hyp_ids,
-                                               [float(scores[j, h]) for h in range(len(hyp_ids))] if return_scores else [])
+                hyps = [[self._target[i] for i in h] for h in hyp_ids]
+                attention = []
+                if keep_attention:
+                    attention = [self._source_attention(out[3][j, h, :len(hyp_ids[h])], len(rows[b]),
+                                                        len(tokens[b]) if is_text[b] else None)
+                                 for h in range(len(hyp_ids))]
+                    if replace_unknowns:
+                        for h, att in zip(hyps, attention):
+                            _replace_unknowns(h, tokens[b], att, self.unk_token)
+                results[b] = TranslationResult(hyps, hyp_ids,
+                                               [float(scores[j, h]) for h in range(len(hyp_ids))] if return_scores else [],
+                                               [a.tolist() for a in attention] if return_attention else [])
         return results
+
+    def _source_attention(self, rows: np.ndarray, input_len: int, original_len: Optional[int]) -> np.ndarray:
+        """The attention rows of one hypothesis over its source (sequence_to_sequence.cc:395-412): cut to the entry's input
+        length, special tokens included; for token sources the columns of the model's added <s> / </s> are dropped and the
+        rows zero-padded to the token count.  Id sources keep the columns of their ids."""
+        rows = rows[:, :input_len]
+        if original_len is None:
+            return rows
+        if self._config.get("add_source_bos", False):
+            rows = rows[:, 1:]
+        if self._config.get("add_source_eos", False):
+            rows = rows[:, :-1]
+        out = np.zeros((rows.shape[0], original_len), np.float32)
+        n = min(original_len, rows.shape[1])
+        out[:, :n] = rows[:, :n]
+        return out
 
     def score_batch(self, source, target, *, max_batch_size: int = 0, batch_type: str = "examples",
                     max_input_length: int = 1024, offset: int = 0, asynchronous: bool = False) -> List[ScoringResult]:
@@ -365,11 +437,17 @@ class Translator:
 
     def translate_ids(self, rows, *, beam_size=2, patience=1.0, num_hypotheses=1, length_penalty=1.0, max_decoding_length=256,
                       min_decoding_length=1, return_end_token=False, end_token=None, start_id: Optional[int] = None,
-                      repetition_penalty=1.0, no_repeat_ngram_size=0, disable_ids=(), suppress_sequences=()):
+                      repetition_penalty=1.0, no_repeat_ngram_size=0, disable_ids=(), suppress_sequences=(),
+                      return_attention=False, coverage_penalty=0.0):
         """ids in, ids out: (ids [batch, num_hypotheses, max_decoding_length], lens, scores [batch, num_hypotheses]).
-        The logits processors take target ids: disable_ids are disabled at every step, suppress_sequences are id lists."""
+        The logits processors take target ids: disable_ids are disabled at every step, suppress_sequences are id lists.
+        return_attention appends the raw attention [batch, num_hypotheses, max_decoding_length, max_source_len] float32:
+        row t of a hypothesis comes from the step that produced token t, zeros past its tokens and past the entry's
+        length.  coverage_penalty (finite) adds the coverage term to the final scores."""
         penalty, ngram, disable_ids, seq_offsets, seq_ids = _processor_options(
             repetition_penalty, no_repeat_ngram_size, disable_ids, suppress_sequences, self._tgt_vocab_size)
+        return_attention = _flag("return_attention", return_attention)
+        coverage = _coverage_penalty(coverage_penalty)
         B = len(rows)
         lens = np.array([len(r) for r in rows], np.int32)
         S = int(lens.max())
@@ -391,6 +469,16 @@ class Translator:
                 ctypes.c_int64(min_decoding_length), int(num_hypotheses), ctypes.c_int32(start_id), end_ids.ctypes.data_as(p),
                 int(end_ids.size), int(return_end_token))
         outs = (out.ctypes.data_as(p), out_lens.ctypes.data_as(p), scores.ctypes.data_as(p))
+        if return_attention or coverage != 0:
+            dis = np.array(disable_ids, np.int32)
+            offsets = np.array(seq_offsets, np.int32)
+            flat = np.array(seq_ids, np.int32)
+            attention = np.zeros((B, num_hypotheses, max_decoding_length, S), np.float32) if return_attention else None
+            check(lib().ct2b200_translate_batch_attention(
+                *args, ctypes.c_float(penalty), int(ngram), dis.ctypes.data_as(p), int(dis.size), flat.ctypes.data_as(p),
+                offsets.ctypes.data_as(p), max(0, int(offsets.size) - 1), ctypes.c_float(coverage), *outs,
+                attention.ctypes.data_as(p) if return_attention else None))
+            return (out, out_lens, scores, attention) if return_attention else (out, out_lens, scores)
         if penalty == 1 and ngram == 0 and not disable_ids and not seq_offsets:
             check(lib().ct2b200_translate_batch(*args, *outs))
         else:

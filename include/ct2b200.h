@@ -433,6 +433,28 @@ CT2B200_API int ct2b200_translate_batch_processors(ct2b200_translator* t, const 
                             float repetition_penalty, int no_repeat_ngram_size, const int32_t* disable_ids_h, int num_disable_ids,
                             const int32_t* sequence_ids_h, const int32_t* sequence_offsets_h, int num_sequences,
                             int32_t* out_ids_h, int32_t* out_lens_h, float* out_scores_h);
+/* ct2b200_translate_batch_processors with the alignment attention of TranslationOptions (return_attention, replace_unknowns and
+ * coverage_penalty; DecodingResult::attention of BeamSearch::search, src/decoding.cc:425-720, and finalize_result, :176-254).
+ * The attention of a step is the mean over heads [0, decoder/alignment_heads) of the softmax-normalised cross-attention of
+ * layer decoder/alignment_layer (src/layers/transformer.cc:518-528, 811-838); the search keeps it for every beam on the
+ * device and follows the beam reordering.
+ *   coverage_penalty (finite; 0 = off): at finalize each score, after the length normalisation, gains
+ *   coverage_penalty * sum over the source positions with coverage > 0 of log(min(coverage, 1)), coverage = the attention
+ *   summed over every row of the hypothesis, end token included (compute_coverage_penalty, decoding.cc:176-187); the
+ *   hypotheses are sorted after that, and early exit is off (:457).
+ *   out_attention_h (null = not returned): [batch, num_hypotheses, max_decoding_length, max_source_len] f32, one row per
+ *   returned token (row t from the decoder step that produced token t; the rows of stripped end tokens go with them,
+ *   sequence_to_sequence.cc:381-391), zeros past the last row and past each entry's source length; the caller trims the
+ *   columns to the source (:395-412).
+ * Neither one asked: the results and the device work are those of ct2b200_translate_batch_processors. */
+CT2B200_API int ct2b200_translate_batch_attention(ct2b200_translator* t, const int32_t* source_ids_h,
+                            const int32_t* source_lens_h, int64_t batch, int64_t max_source_len, int beam_size, float patience,
+                            float length_penalty, int64_t max_decoding_length, int64_t min_decoding_length, int num_hypotheses,
+                            int32_t start_id, const int32_t* end_ids_h, int num_end_ids, int return_end_token,
+                            float repetition_penalty, int no_repeat_ngram_size, const int32_t* disable_ids_h, int num_disable_ids,
+                            const int32_t* sequence_ids_h, const int32_t* sequence_offsets_h, int num_sequences,
+                            float coverage_penalty, int32_t* out_ids_h, int32_t* out_lens_h, float* out_scores_h,
+                            float* out_attention_h);
 /* Host only (no device): the per-entry bookkeeping of one BeamSearch::search step (decoding.cc:595-663) — the SAME function the
  * device kernel runs (csrc/kernels/beam_decide.h).  words_h [2 * beam_size] = the candidates' tokens in TopK order.  Outputs:
  * active_h [beam] (candidate each next beam continues), hyp_slot_h / hyp_len_h [beam] (hypothesis registered for candidate k, or

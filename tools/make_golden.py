@@ -421,6 +421,116 @@ def make_seq2seq_processors_fixture():
     print("seq2seq processors fixture:", sum(len(m["cases"]) for e in fixture.values() for m in e["models"].values()), "cases")
 
 
+def ref_translate_attention(model_dir, compute, requests):
+    """Translator::translate_batch of the unmodified reference (CPU) with return_attention, replace_unknowns and
+    coverage_penalty, through tools/ref_translate_attention.cc, built by tools/ref_translate_attention.mk against
+    oracle/_ref/libct2ref.so into a temporary directory.  requests: dicts of sources (token lists), beam_size,
+    num_hypotheses, length_penalty, max_length, min_length, coverage_penalty, return_end_token, return_attention,
+    replace_unknowns.  Per request: per source (hypotheses as token lists, scores, attention [hyp][row][column]), or the
+    reference's error message."""
+    import subprocess
+    import tempfile
+    out_dir = os.path.join(tempfile.gettempdir(), "ct2ref_attention")
+    subprocess.run(["make", "-s", "-f", "tools/ref_translate_attention.mk", "attention", "ATTN_OUT=" + out_dir], cwd=ROOT,
+                   check=True)
+    text = "%s\t%s\n" % (model_dir, compute)
+    for r in requests:
+        text += "\t".join(str(x) for x in (r["beam_size"], r["num_hypotheses"], r["length_penalty"], r["max_length"],
+                                           r["min_length"], r["coverage_penalty"], int(r["return_end_token"]),
+                                           int(r["return_attention"]), int(r["replace_unknowns"]),
+                                           "|".join(" ".join(x) for x in r["sources"]))) + "\n"
+    lines = subprocess.run([os.path.join(out_dir, "ref_translate_attention")], input=text.encode(), capture_output=True,
+                           check=True).stdout.decode().split("\n")
+    res, k = [], 0
+    for r in requests:
+        if lines[k].startswith("ERROR\t"):
+            res.append(lines[k].split("\t", 1)[1])
+            k += 1
+            continue
+        entry = []
+        for _ in r["sources"]:
+            hyps, scores, attn = lines[k].split("\t")
+            matrices = [[[float(x) for x in row.split(" ")] if row else [] for row in m.split(";")] if m else []
+                        for m in attn.split("|")] if attn else []
+            entry.append(([h.split(" ") if h else [] for h in hyps.split("|")], [float(x) for x in scores.split(" ")],
+                          matrices))
+            k += 1
+        res.append(entry)
+    return res
+
+
+ATTENTION_BEAMS = [(1, 1), (2, 2), (4, 3), (10, 2)]   # (beam, num_hypotheses); beam 10 takes the LogSoftMax + TopK path
+
+
+def find_unk_source(path, compute, src_vocab, lo, hi, max_length):
+    """A source of the random model's inputs for which the reference emits <unk> at beam 2."""
+    rng = np.random.default_rng(500)
+    pool = [[src_vocab[int(i)] for i in rng.integers(lo, hi, size=int(rng.integers(3, 10)))] for _ in range(400)]
+    req = dict(sources=pool, beam_size=2, num_hypotheses=1, length_penalty=1.0, max_length=max_length, min_length=1,
+               coverage_penalty=0.0, return_end_token=False, return_attention=False, replace_unknowns=False)
+    for src, out in zip(pool, ref_translate_attention(path, compute, [req])[0]):
+        if "<unk>" in out[0][0]:
+            return src
+    raise RuntimeError("no source of the pool makes the reference emit <unk>")
+
+
+# (length_penalty, coverage_penalty) of each beam size; return_end_token alternates along the list
+ATTENTION_PENALTIES = [(1.0, 0.0), (0.0, 0.2), (1.0, 1.0), (0.0, 0.0), (1.0, 0.2), (0.0, 1.0)]
+
+
+def make_seq2seq_attention_fixture():
+    """Translator::translate_batch with return_attention, replace_unknowns and coverage_penalty, from the UNMODIFIED
+    reference (oracle/_ref, CPU) in float32, on aren-transliteration (default alignment heads), the post-norm model and
+    tiny_seq2seq_align (the post-norm recipe with alignment_layer 0 and alignment_heads 0: the mean over every head of the
+    first layer): beams 1 / 2 / 4 / 10, coverage_penalty 0 / 0.2 / 1 under length_penalty 1 and 0, return_end_token both
+    ways, and a source the reference translates with <unk>, replace_unknowns both ways.
+
+    Beam 1 runs a ragged batch (its padding columns are zeros) and returns the attention of every case (the reference's
+    GreedySearch keeps no attention for a coverage penalty alone, decoding.cc:819-833).  Beam searches run one source per
+    request: at the first step of a beam search over several sources the reference gathers the unexpanded attention with
+    batch indices after repeat_batch expanded it (decoding.cc:565, 590-595), so entry i of its length-sorted batch gets the
+    first row of entry i / beam_size (DESIGN §8).  They return the attention of two penalty settings out of six; the others
+    pin the ranking the coverage penalty makes."""
+    from ctranslate2_b200.converters.synthetic import TransformerConfig, write_transformer_model
+    from ctranslate2_b200.translator import _load_vocabulary
+    align = os.path.join(OUT, "tiny_seq2seq_align")
+    cfg = TransformerConfig(encoder_layers=2, decoder_layers=2, num_heads=4, d_model=64, ffn_dim=128, source_vocab=120,
+                            target_vocab=96, pre_norm=False, activation=2, start_from_zero_embedding=True)
+    write_transformer_model(align, cfg, "int8", seed=7, alignment_layer=0, alignment_heads=0)
+    max_length = 10
+    fixture = {}
+    for name, mdir, lo, hi in (("aren", "aren-transliteration", 4, 51), ("postnorm", "tiny_seq2seq_postnorm", 3, 120),
+                               ("align", "tiny_seq2seq_align", 3, 120)):
+        path = os.path.join(OUT, mdir)
+        src_vocab = _load_vocabulary(path, "source_vocabulary")
+        srcs = [[src_vocab[i] for i in r] for r in seq2seq_sources(310, 1, lo, hi)[0]]
+        srcs = (srcs + [[src_vocab[i] for i in r] for r in seq2seq_sources(311, 1, lo, hi)[0]])[:3]
+        base = dict(min_length=1, max_length=max_length, replace_unknowns=False)
+        requests = []
+        for beam, nh in ATTENTION_BEAMS:
+            for k, (lp, cov) in enumerate(ATTENTION_PENALTIES):
+                requests.append(dict(base, sources=srcs if beam == 1 else [srcs[k % len(srcs)]], beam_size=beam,
+                                     num_hypotheses=nh, length_penalty=lp, coverage_penalty=cov, return_end_token=k % 2 == 1,
+                                     return_attention=beam == 1 or k in (1, 2)))
+        if name != "aren":                          # the aren vocabularies have no <unk>
+            unk = find_unk_source(path, "float32", src_vocab, lo, hi, max_length)
+            for beam, nh in ((1, 1), (2, 2)):
+                for ret_attn in (False, True):
+                    for rep in (False, True):
+                        requests.append(dict(base, sources=[unk, srcs[0]] if beam == 1 else [unk], beam_size=beam,
+                                             num_hypotheses=nh, length_penalty=1.0, coverage_penalty=0.0,
+                                             return_end_token=False, return_attention=ret_attn, replace_unknowns=rep))
+        res = ref_translate_attention(path, "float32", requests)
+        cases = []
+        for r, out in zip(requests, res):
+            assert not isinstance(out, str), out
+            cases.append(dict(r, hypotheses=[o[0] for o in out], scores=[o[1] for o in out], attention=[o[2] for o in out]))
+        fixture[name] = {"model": mdir, "compute_type": "float32", "cases": cases}
+    with open(os.path.join(OUT, "seq2seq_attention_ref.json"), "w") as f:
+        json.dump(fixture, f, ensure_ascii=False, separators=(",", ":"))
+    print("seq2seq attention fixture:", sum(len(e["cases"]) for e in fixture.values()), "cases")
+
+
 WHISPER_CASES = [  # (beam, num_hypotheses, length_penalty, max_length, suppress_blank, timestamps)
     (1, 1, 1.0, 24, True, False), (3, 2, 1.0, 24, True, False), (5, 3, 1.0, 30, True, False), (5, 1, 0.0, 24, False, False),
     (2, 2, 0.7, 16, True, False), (1, 1, 1.0, 30, True, True), (5, 2, 1.0, 30, True, True), (3, 3, 1.0, 24, False, True)]
@@ -727,6 +837,9 @@ def main():
     if "--processors-only" in sys.argv:
         make_processors_fixture()
         return
+    if "--seq2seq-attention-only" in sys.argv:
+        make_seq2seq_attention_fixture()
+        return
     if "--gtest-only" in sys.argv:
         with open(os.path.join(OUT, "ref_gtest_vectors.json"), "w") as f:
             json.dump(extract_gtest_vectors(), f)
@@ -797,6 +910,7 @@ def main():
     make_seq2seq_fixture()
     make_translator_score_fixture()
     make_seq2seq_processors_fixture()
+    make_seq2seq_attention_fixture()
     make_whisper_fixture()
     make_whisper_align_fixture()
     make_whisper_sampling_fixture()
